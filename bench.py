@@ -5,13 +5,14 @@ Flagship step = BASELINE.json config "4096x4096 linear layer: Allreduce(params)
 -> GEMM fused, loss Allreduce backward": every rank holds a 4096x4096 bf16
 weight and a private batch; one step is, THROUGH THE AUTOGRAD GRAPH,
 
-    local = dp_linear_mse(x, W, t)            Allreduce(W)/size -> tcgen05 GEMM -> MSE epilogue
+    local = dp_linear_mse(x, W, t)            Allreduce(W)/size -> wgmma GEMM -> MSE epilogue
     loss  = comm.Allreduce(local, MPI_SUM)    the library's differentiable Allreduce
     loss.backward()                           adjoint Allreduce of the scalar, wgrad GEMM, adjoint
                                               Allreduce of dW fused with the SGD update
 
     python bench.py --gpus N --steps K --warmup W            (N>1: under torchrun)
     python bench.py --impl reference ...                      (the unmodified reference, baseline/)
+    python bench.py ... --dump-outputs DIR                    (also write the last timed step's results as .npy)
 
 Prints ONE JSON line on rank 0.  `value` = samples/s over the whole job, timed on the device (CUDA
 events, max over ranks); `e2e` = the same step through the public API including per-step H2D of the
@@ -35,7 +36,8 @@ if ROOT not in sys.path:
 METRIC = "dp_linear4096_train_samples_per_s"
 IN_F = OUT_F = 4096
 PER_GPU_BATCH = 8192
-POOL = 4  # rotating input batches: 4 x (64 MiB x + 64 MiB t) >> 126 MB L2
+POOL = 4  # rotating input batches: 4 x (64 MiB x + 64 MiB t) >> 50 MB L2
+DUMP_WEIGHT_SAMPLE = 1 << 20  # weight elements written by --dump-outputs (4 MiB as float32)
 
 
 def linreg_cpu_step_per_s() -> object:
@@ -55,6 +57,20 @@ def linreg_cpu_step_per_s() -> object:
         return {"error": f"{type(exc).__name__}: {exc}"[:200]}
 
 
+def dump_outputs(out_dir: str, loss, weight) -> None:
+    """The results of the last timed step as a caller sees them: the loss and the updated weight (a fixed,
+    seeded sample of its elements, the same indices on every run), both as float32 .npy files."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    idx = torch.randint(0, weight.numel(), (min(DUMP_WEIGHT_SAMPLE, weight.numel()),),
+                        generator=torch.Generator().manual_seed(0))
+    w = weight.detach().reshape(-1)[idx.to(weight.device)].float().cpu().numpy()
+    np.save(os.path.join(out_dir, "loss.npy"), np.asarray([float(loss)], dtype=np.float32))
+    np.save(os.path.join(out_dir, "weight_sample.npy"), w.astype(np.float32))
+
+
 def main() -> int:
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -67,6 +83,8 @@ def main() -> int:
     ap.add_argument("--unfused", action="store_true", help="force the unfused Allreduce + GEMM composition")
     ap.add_argument("--plain-sgd", action="store_true", help="weight.grad + separate SGD instead of the optimizer in backward")
     ap.add_argument("--full-sweep", action="store_true", help="1 KiB .. 1 GiB in x4 steps instead of the quick table")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (loss, seeded sample of the updated weight) as .npy")
     args = ap.parse_args()
     if args.impl == "reference":
         sys.path.insert(0, os.path.join(ROOT, "baseline"))
@@ -147,6 +165,8 @@ def main() -> int:
     table0 = dict(_C.kernel_launch_table())
     dev_ms, launches, loss = timed(step, args.steps, 0)
     final_loss = float(loss)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, loss, model.weight)
     # which tensor-core / fused kernels really ran in the timed region (launches per step)
     path = {k: (v - table0.get(k, 0)) / args.steps for k, v in dict(_C.kernel_launch_table()).items()
             if v - table0.get(k, 0) > 0}
@@ -231,7 +251,7 @@ def main() -> int:
             "seq_len": 1,
             "parallelism": f"dp{size}",
             "per_gpu_batch": B,
-            "cold_cache": f"inputs rotate over {POOL} batches (>= {POOL * 2 * B * IN_F * 2 >> 20} MiB) > 126 MB L2",
+            "cold_cache": f"inputs rotate over {POOL} batches (>= {POOL * 2 * B * IN_F * 2 >> 20} MiB) > 50 MB L2",
             "autograd": True,
             "optimizer_in_backward": bool(model.sgd_in_backward and model._in_backward(xs[0])),
             "kernels_per_step": path,

@@ -2,7 +2,7 @@
 """Allreduce forward+backward bus-bandwidth sweep, 1 KiB .. 1 GiB bf16
 (BASELINE.json config 2), ours next to the comparators BASELINE.md names:
 
-  ours     hand-written sm_100a kernels over the symmetric heap (this library)
+  ours     hand-written sm_90a kernels over the symmetric heap (this library)
   nccl     NCCL through torch.distributed, wrapped in the same autograd adjoint
   staged   host-staged: D2H -> CPU shared-memory reduce -> H2D  (what the
            reference does without a CUDA-aware MPI, csrc/extension.cpp:75-89)

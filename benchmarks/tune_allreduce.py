@@ -32,7 +32,7 @@ def timeit(fn, iters=5, warm=2):
 
 
 sizes = [int(s) for s in os.environ.get("TUNE_SIZES", f"{64 << 20},{256 << 20}").split(",")]
-blocks_list = [int(s) for s in os.environ.get("TUNE_BLOCKS", "32,64,128,148,296").split(",")]
+blocks_list = [int(s) for s in os.environ.get("TUNE_BLOCKS", "32,64,128,132,264").split(",")]
 chunks = [int(s) for s in os.environ.get("TUNE_CHUNKS_KB", "1024,4096,16384,1048576").split(",")]
 algos = [int(s) for s in os.environ.get("TUNE_ALGOS", "3,2").split(",")]
 for nbytes in sizes:

@@ -1,4 +1,4 @@
-"""mpi4torch_b200 - B200-native, autodiff-transparent collectives for PyTorch.
+"""mpi4torch_b200 - H100-native, autodiff-transparent collectives for PyTorch.
 
 API parity with helmholtz-analytics/mpi4torch (reference ``src/__init__.py``):
 ``COMM_WORLD``, ``MPI_Communicator`` with ``Allreduce / Bcast_ / Reduce_ /
@@ -13,8 +13,8 @@ whose backward is the adjoint communication.  Added on top: ``Reduce_scatter``
 
 There is no MPI underneath.  Ranks are OS processes started by
 ``python -m mpi4torch_b200.launch`` (or ``torchrun``); CPU tensors travel over a
-POSIX shared-memory backend, CUDA tensors over hand-written sm_100a kernels
-that read and write peer GPUs' HBM through NVLink 5 / NVSwitch (NVLS multicast
+POSIX shared-memory backend, CUDA tensors over hand-written sm_90a kernels
+that read and write peer GPUs' HBM through NVLink 4 / NVSwitch (NVLS multicast
 when the fabric offers it).
 """
 from __future__ import annotations

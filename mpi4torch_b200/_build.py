@@ -1,9 +1,9 @@
-"""In-tree build of the native core (C++ runtime + sm_100a kernels).
+"""In-tree build of the native core (C++ runtime + sm_90a kernels).
 
 The reference builds one C++ TU through ``mpicc``/``mpicxx`` with ``-g`` only
 (reference ``setup.py:22-58``, ``:90-106``).  Here the extension is a mix of
 plain C++ (control plane, CPU backend, symmetric heap), torch-facing C++
-(autograd layer, bindings) and CUDA compiled **only** for sm_100a.  The built
+(autograd layer, bindings) and CUDA compiled **only** for sm_90a.  The built
 ``.so`` lives in ``mpi4torch_b200/_lib`` so it travels with the source tree; a
 content hash of sources + flags decides whether it is stale.
 """
@@ -36,9 +36,8 @@ _SOURCES = [
     "kernels/slab_push.cu",
     "kernels/rooted.cu",
     "kernels/p2p.cu",
-    "kernels/gemm_tcgen05.cu",
-    "kernels/gemm_tcgen05_2cta.cu",
-    "kernels/wgrad_tcgen05_2cta.cu",
+    "kernels/gemm_wgmma.cu",
+    "kernels/wgrad_wgmma.cu",
     "api/comm_raw.cpp",
     "api/autograd_ops.cpp",
     "api/fused_ops.cpp",
@@ -51,7 +50,7 @@ NVCC_FLAGS = [
     "-O3",
     "-std=c++17",
     "-gencode",
-    "arch=compute_100a,code=sm_100a",
+    "arch=compute_90a,code=sm_90a",
     "-lineinfo",
     "--expt-relaxed-constexpr",
     "-diag-suppress",
@@ -109,6 +108,7 @@ def build(verbose: bool = False, force: bool = False):
         return _import_built()
     from torch.utils import cpp_extension
 
+    stamp = _stamp()  # of the sources being compiled, not of whatever is on disk when the compile ends
     _LIB.mkdir(exist_ok=True)
     os.environ.setdefault("MAX_JOBS", str(os.cpu_count() or 8))
     # The image presets CXX=/opt/gcc/bin/g++, a wrapper whose libstdc++.so symlink
@@ -129,7 +129,7 @@ def build(verbose: bool = False, force: bool = False):
         is_python_module=True,
         verbose=verbose,
     )
-    (_LIB / ".stamp").write_text(_stamp())
+    (_LIB / ".stamp").write_text(stamp)
     return sys.modules.get(_NAME) or _import_built()
 
 

@@ -1,4 +1,4 @@
-// Tensor-core ops exposed to Python: the tcgen05 GEMM and the fused
+// Tensor-core ops exposed to Python: the wgmma GEMM and the fused
 // Allreduce->GEMM linear forward (BASELINE.json config "4096x4096 linear layer:
 // Allreduce(params)->GEMM fused").  The reference has no fused op and no GPU
 // kernel at all (SURVEY 2.4); its equivalent is Allreduce + `/ size` + matmul
@@ -29,7 +29,7 @@ void check_2d_bf16(const Tensor& t, const char* name) {
               "mpi4torch_b200: ", name, " must be a 2-d bf16 CUDA tensor with unit inner stride");
 }
 
-// y = x @ w^T on the tcgen05 path.
+// y = x @ w^T on the wgmma path.
 Tensor gemm_bf16_tn(const Tensor& x, const Tensor& w) {
   check_2d_bf16(x, "x");
   check_2d_bf16(w, "w");
@@ -43,7 +43,7 @@ Tensor gemm_bf16_tn(const Tensor& x, const Tensor& w) {
   return y;
 }
 
-// Same GEMM on CTA pairs (cta_group::2); exposed separately for A/B testing.
+// Same GEMM on CTA pairs (clusters of two sharing the B tile by TMA multicast); exposed separately for A/B testing.
 Tensor gemm_bf16_tn_2cta(const Tensor& x, const Tensor& w) {
   check_2d_bf16(x, "x");
   check_2d_bf16(w, "w");
@@ -59,7 +59,7 @@ Tensor gemm_bf16_tn_2cta(const Tensor& x, const Tensor& w) {
 }
 
 // y = a @ b with both operands row-major (dgrad: gy[M,N] @ W[N,K]); the weight is read in place through an
-// MN-major tcgen05 operand, no transposed copy.
+// MN-major wgmma operand, no transposed copy.
 bool gemm_bf16_nn_ok(const Tensor& a, const Tensor& b) {
   if (!(a.is_cuda() && b.is_cuda() && a.dim() == 2 && b.dim() == 2 && a.scalar_type() == at::kBFloat16 &&
         b.scalar_type() == at::kBFloat16 && a.stride(1) == 1 && b.stride(1) == 1 && a.size(1) == b.size(0)))
@@ -77,9 +77,9 @@ Tensor gemm_bf16_nn(const Tensor& a, const Tensor& b) {
   Tensor y = at::empty({a.size(0), b.size(1)}, a.options());
   if (y.numel() == 0) return y;
   std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
-  launch_gemm_bf16_nn_2cta(a.data_ptr(), b.data_ptr(), y.data_ptr(), a.size(0), b.size(1), a.size(1), a.stride(0),
-                           b.stride(0), y.stride(0), backend().device_comm().sm_count,
-                           c10::cuda::getCurrentCUDAStream(a.device().index()).stream());
+  launch_gemm_bf16_nn(a.data_ptr(), b.data_ptr(), y.data_ptr(), a.size(0), b.size(1), a.size(1), a.stride(0),
+                      b.stride(0), y.stride(0), backend().device_comm().sm_count,
+                      c10::cuda::getCurrentCUDAStream(a.device().index()).stream());
   return y;
 }
 
@@ -116,7 +116,7 @@ std::tuple<Tensor, Tensor> allreduce_linear_fused(const Tensor& x, const Tensor&
 
 // Training forward of the data-parallel linear layer with everything fused:
 //   W_avg = scale * sum_ranks W          (inside the GEMM kernel when NVLS is up)
-//   y     = x @ W_avg^T                  (tcgen05, never stored)
+//   y     = x @ W_avg^T                  (wgmma, never stored)
 //   dy    = grad_scale * (y - target)    (GEMM epilogue)
 //   loss  = loss_scale * sum((y-target)^2)  (GEMM epilogue, one atomic per warp per tile)
 // Returns (dy, loss[1] fp32, W_avg).
@@ -190,7 +190,7 @@ const float* grad_scale_ptr(const c10::optional<Tensor>& gs, const Tensor& like)
   return gs->data_ptr<float>();
 }
 
-// G = grad_scale * dy^T @ x on the tcgen05 path with MN-major operands (no transposed copies).
+// G = grad_scale * dy^T @ x on the wgmma path with MN-major operands (no transposed copies).
 // grad_scale is a device scalar (the upstream gradient of the loss as autograd delivers it).
 Tensor wgrad_bf16(const Tensor& dy, const Tensor& x, const c10::optional<Tensor>& grad_scale) {
   check_2d_bf16(dy, "dy");

@@ -1,7 +1,7 @@
 #include <map>
 #include <mutex>
 #include <string>
-// Allreduce over NVLink 5 / NVSwitch: one launch per collective, forward AND
+// Allreduce over NVLink 4 / NVSwitch: one launch per collective, forward AND
 // backward (the adjoint of Allreduce(SUM) is Allreduce(SUM), reference
 // csrc/extension.cpp:265-272), with the adjacent elementwise work fused in:
 //   out = accumulate + scale * reduce_ranks(in)        (cast in the store)

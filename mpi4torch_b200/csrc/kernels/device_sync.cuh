@@ -25,7 +25,7 @@
 
 namespace m4t {
 
-constexpr int kMaxGpuPeers = 16;       // one NVLink domain (8 on HGX B200)
+constexpr int kMaxGpuPeers = 16;       // one NVLink domain (8 on HGX H100)
 constexpr int kMaxChannels = 512;      // barrier channels == max grid of barrier kernels
 constexpr int kErrTimeout = 1;
 

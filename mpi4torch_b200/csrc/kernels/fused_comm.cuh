@@ -2,7 +2,7 @@
 // panel by panel through the NVSwitch (multimem.ld_reduce -> x scale ->
 // multimem.st into every rank's W_avg -> multimem.red on the panel counter) so
 // that the tensor-core warps of the same kernel can consume finished panels.
-// Shared by the single-CTA and the CTA-pair GEMM kernels.
+// Used by the fused kernel of gemm_wgmma.cu.
 #pragma once
 #include "device_sync.cuh"
 #include "vec_ops.cuh"

@@ -1,0 +1,358 @@
+// wgmma GEMM for the linear layer:  C[M,N] = A[M,K] * B[N,K]^T   (bf16 in, fp32
+// accumulate in registers, bf16 out), its dgrad form C = A[M,K] * B[K,N] (B read
+// MN-major in place), and the fused form where the B operand is the rank-average of
+// every rank's weight and is produced INSIDE the same kernel by communication warps
+// (fused_allreduce_gemm, below).
+//
+// Structure: see wgmma_pipeline.cuh (persistent CTAs, 128x256 tiles - 128x128 in the fused
+// kernel -, TMA producer warp, two consumer warpgroups; CL = 2: CTA pairs in a cluster on
+// 256x256 tiles, B multicast).  Fused kernel only: four communication warps run the NVLS
+// reduce of weight panels (multimem.ld_reduce over all ranks' weights -> x 1/size ->
+// multimem.st into every rank's W_avg -> multimem.red on the panel counter).  The TMA
+// producer polls that counter before loading from a panel, so the all-reduce of panel
+// p+1.. overlaps the MMAs on panel p.
+#include <cuda.h>
+
+#include <algorithm>
+#include <mutex>
+
+#include "kernels.h"
+#include "fused_comm.cuh"
+#include "tma_host.h"
+#include "wgmma_pipeline.cuh"
+
+namespace m4t {
+
+namespace {
+
+using namespace wg;
+
+constexpr int kPanel = 256;  // weight rows per all-reduce panel of the fused kernel (one counter each)
+constexpr int kCommWarps = 4;
+
+struct GemmArgs {
+  void* C;
+  int M, N, K;
+  int ldc;
+  // fused MSE epilogue (EPI == 1): C receives dL/dy = grad_scale * (y - T),
+  // loss_acc accumulates loss_scale * sum((y - T)^2); y itself is never stored
+  const void* T;
+  int ldt;
+  float* loss_acc;
+  float loss_scale, grad_scale;
+  // fused mode ----------------------------------------------------------------
+  const uint32_t* panel_flags;  // [N / kPanel] counters in local HBM (written through multicast)
+  uint32_t panel_target;        // a panel is ready when its counter >= target (wrap-safe)
+};
+
+// the fused kernel's communication warps need registers: half-width tiles there
+template <bool FUSED> constexpr int tile_n() { return FUSED ? 128 : 256; }
+
+// CL = 2: launched as clusters of two CTAs (launch_pair below); each pair works on 256-row tiles.
+template <bool FUSED, int EPI, bool B_MN, int CL = 1>
+__global__ void __launch_bounds__(kGemmThreads + (FUSED ? kCommWarps * 32 : 0), 1)
+gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                       const GemmArgs g, const CommArgs cm) {
+  static_assert(CL == 1 || !FUSED, "the fused kernel runs on single CTAs");
+  constexpr int BN = tile_n<FUSED>();
+  constexpr int TM = BM * CL;  // rows of a tile
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = aligned_smem(smem_raw);
+  Pipe* pipe = pipe_of<BN>(smem);
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const uint32_t crank = CL == 2 ? tc::cluster_ctarank() : 0u;
+  const int group = blockIdx.x / CL, num_groups = gridDim.x / CL;  // both CTAs of a pair walk the same tiles
+
+  const int m_tiles = (g.M + TM - 1) / TM;
+  const int n_tiles = (g.N + BN - 1) / BN;
+  const int num_tiles = m_tiles * n_tiles;
+  const int k_blocks = (g.K + BK - 1) / BK;
+
+  if (warp == 0 && lane == 0) {
+    tc::prefetch_tmap(&tmap_a);
+    tc::prefetch_tmap(&tmap_b);
+    init_pipe<BN, CL>(pipe);
+  }
+  if (CL == 2) tc::cluster_sync();  // the peer's barriers exist before anything is multicast into them
+  else __syncthreads();
+
+  if (warp < 4) {
+    // =========================== TMA producer ===========================
+    if (warp == 0 && lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int t = group; t < num_tiles; t += num_groups) {
+        const int n_blk = t / m_tiles;  // M fastest: a wave works on few weight panels
+        const int m_blk = t - n_blk * m_tiles;
+        if (FUSED) {
+          // the weight panel must have been all-reduced (by every rank) first
+          const uint32_t* flag = g.panel_flags + n_blk * BN / kPanel;
+          // bounded like every other cross-rank wait: a peer that never publishes
+          // must end in an error, not in a hung GPU
+          if (static_cast<int32_t>(ld_acquire_sys_u32(flag) - g.panel_target) < 0) {
+            const unsigned long long t0 = globaltimer_ns();
+            unsigned int spins = 0;
+            while (static_cast<int32_t>(ld_acquire_sys_u32(flag) - g.panel_target) < 0) {
+              if ((++spins & 0x3ff) == 0 && globaltimer_ns() - t0 > cm.sync.timeout_ns) {
+                *reinterpret_cast<volatile int*>(cm.sync.err_flag) = kErrTimeout;
+                __threadfence_system();
+                __trap();
+              }
+            }
+          }
+          tc::fence_proxy_async();  // generic-proxy writes (multimem.st) -> async-proxy reads (TMA)
+        }
+        for (int kb = 0; kb < k_blocks; ++kb)
+          load_stage<false, B_MN, BN, CL>(smem, pipe, stage, phase, &tmap_a, &tmap_b, m_blk * TM + crank * BM, n_blk * BN,
+                                          kb * BK, crank);
+      }
+    }
+  } else if (warp < kGemmThreads / 32) {
+    // ====================== consumers: wgmma + epilogue ======================
+    const int wgi = warp / 4 - 1;
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[BN / 2];
+    for (int t = group; t < num_tiles; t += num_groups) {
+      const int n_blk = t / m_tiles;
+      const int m_blk = t - n_blk * m_tiles;
+      mma_tile<false, B_MN, BN, CL>(acc, smem, pipe, stage, phase, k_blocks, wgi, crank);
+      float loss_part = 0.f;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = m_blk * TM + static_cast<int>(crank) * BM + wgi * 64 + frag_row(h);
+        if (row >= g.M) continue;
+        uint16_t* crow = static_cast<uint16_t*>(g.C) + static_cast<int64_t>(row) * g.ldc;
+        const uint16_t* trow = EPI == 1 ? static_cast<const uint16_t*>(g.T) + static_cast<int64_t>(row) * g.ldt : nullptr;
+        // N is a multiple of 8, so a column pair is either wholly inside or wholly outside
+#pragma unroll
+        for (int j0 = 0; j0 < BN / 8; j0 += 8) {
+          uint32_t tv[8];  // the targets of eight column pairs are requested before the first is used
+          if (EPI == 1) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const int col = n_blk * BN + frag_col(j0 + j);
+              tv[j] = col < g.N ? __ldcs(reinterpret_cast<const unsigned int*>(trow + col)) : 0u;
+            }
+          }
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const int col = n_blk * BN + frag_col(j0 + j);
+            if (col >= g.N) continue;
+            float v0 = acc[4 * (j0 + j) + 2 * h], v1 = acc[4 * (j0 + j) + 2 * h + 1];
+            if (EPI == 1) {
+              const float d0 = v0 - bf16_bits_to_float(static_cast<uint16_t>(tv[j] & 0xffffu));
+              const float d1 = v1 - bf16_bits_to_float(static_cast<uint16_t>(tv[j] >> 16));
+              loss_part = fmaf(d0, d0, loss_part);
+              loss_part = fmaf(d1, d1, loss_part);
+              v0 = d0 * g.grad_scale;
+              v1 = d1 * g.grad_scale;
+            }
+            *reinterpret_cast<uint32_t*>(crow + col) = pack_bf16x2(v0, v1);
+          }
+        }
+      }
+      if (EPI == 1) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) loss_part += __shfl_xor_sync(0xffffffffu, loss_part, o);
+        if (lane == 0) atomicAdd(g.loss_acc, loss_part * g.loss_scale);
+      }
+    }
+  } else if (FUSED) {
+    // =========================== communication ==========================
+    comm_allreduce_panels<kCommWarps, kPanel>(cm, kGemmThreads, g.N / kPanel, g.K);
+  }
+  if (CL == 2) tc::cluster_sync();  // the peer may still multicast into / arrive on this CTA's barriers
+  else __syncthreads();
+}
+
+// ---------------------------------------------------------------------------
+// host side
+// ---------------------------------------------------------------------------
+// Row-major [rows, cols] bf16 matrix, box = [box_rows, 64 cols], 128-byte swizzle.
+CUtensorMap make_tmap(const void* base, int64_t rows, int64_t cols, int64_t ld, int box_rows) {
+  return make_tmap_bf16_sw128(base, rows, cols, ld, BK, box_rows);
+}
+
+template <bool FUSED> constexpr int smem_bytes() { return Tile<tile_n<FUSED>()>::kSmemBytes; }
+
+template <bool FUSED, int EPI, bool B_MN, int CL = 1> void configure_once() {
+  static std::once_flag once;
+  std::call_once(once, [] {
+    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<FUSED, EPI, B_MN, CL>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes<FUSED>());
+    M4T_CHECK(e == cudaSuccess, "cudaFuncSetAttribute(smem) failed: " << cudaGetErrorString(e));
+  });
+}
+
+template <bool FUSED, int EPI, bool B_MN>
+void launch(int grid, const CUtensorMap& ta, const CUtensorMap& tb, const GemmArgs& g, const CommArgs& cm,
+            cudaStream_t stream, const char* what) {
+  configure_once<FUSED, EPI, B_MN>();
+  gemm_bf16_wgmma_kernel<FUSED, EPI, B_MN>
+      <<<grid, kGemmThreads + (FUSED ? kCommWarps * 32 : 0), smem_bytes<FUSED>(), stream>>>(ta, tb, g, cm);
+  cudaError_t e = cudaGetLastError();
+  M4T_CHECK(e == cudaSuccess, what << " launch failed: " << cudaGetErrorString(e));
+  note_kernel_launch(what);
+}
+
+// Clusters of two CTAs (`pairs` of them) for the CL = 2 kernel.
+template <int EPI>
+void launch_pair(int pairs, const CUtensorMap& ta, const CUtensorMap& tb, const GemmArgs& g, cudaStream_t stream,
+                 const char* what) {
+  configure_once<false, EPI, false, 2>();
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(2 * pairs, 1, 1);
+  cfg.blockDim = dim3(kGemmThreads, 1, 1);
+  cfg.dynamicSmemBytes = smem_bytes<false>();
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = 2;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  cudaError_t e = cudaLaunchKernelEx(&cfg, gemm_bf16_wgmma_kernel<false, EPI, false, 2>, ta, tb, g, CommArgs{});
+  M4T_CHECK(e == cudaSuccess, what << " launch failed: " << cudaGetErrorString(e));
+  e = cudaGetLastError();
+  M4T_CHECK(e == cudaSuccess, what << " launch failed: " << cudaGetErrorString(e));
+  note_kernel_launch(what);
+}
+
+void set_mse(GemmArgs& g, const MseEpilogue* mse) {
+  g.T = mse->target;
+  g.ldt = static_cast<int>(mse->ldt);
+  g.loss_acc = mse->loss_acc;
+  g.loss_scale = mse->loss_scale;
+  g.grad_scale = mse->grad_scale;
+}
+
+}  // namespace
+
+bool gemm_bf16_tn_supported(int64_t M, int64_t N, int64_t K, const void* A, const void* B, const void* C, int64_t lda,
+                            int64_t ldb, int64_t ldc) {
+  auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
+  return M > 0 && N > 0 && K > 0 && (K % 8) == 0 && (N % 8) == 0 && (lda % 8) == 0 && (ldb % 8) == 0 && (ldc % 8) == 0 &&
+         al16(A) && al16(B) && al16(C) && M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31);
+}
+
+void launch_gemm_bf16_tn(const void* A, const void* B, void* C, int64_t M, int64_t N, int64_t K, int64_t lda,
+                         int64_t ldb, int64_t ldc, int sm_count, cudaStream_t stream, const MseEpilogue* mse) {
+  M4T_CHECK(gemm_bf16_tn_supported(M, N, K, A, B, C, lda, ldb, ldc), "unsupported GEMM shape/alignment for the wgmma path");
+  constexpr int BN = tile_n<false>();
+  const CUtensorMap ta = make_tmap(A, M, K, lda, BM);
+  const CUtensorMap tb = make_tmap(B, N, K, ldb, BN);
+  GemmArgs g{};
+  g.C = C;
+  g.M = static_cast<int>(M);
+  g.N = static_cast<int>(N);
+  g.K = static_cast<int>(K);
+  g.ldc = static_cast<int>(ldc);
+  const int tiles = static_cast<int>(((M + BM - 1) / BM) * ((N + BN - 1) / BN));
+  const int grid = std::max(1, std::min(tiles, sm_count));
+  if (mse) {
+    set_mse(g, mse);
+    launch<false, 1, false>(grid, ta, tb, g, CommArgs{}, stream, "gemm_mse_epilogue");
+  } else {
+    launch<false, 0, false>(grid, ta, tb, g, CommArgs{}, stream, "gemm_bf16_tn");
+  }
+}
+
+// Same contract on CTA pairs: 256x256 tiles, each CTA loads half of the B tile and multicasts it to both.
+void launch_gemm_bf16_tn_2cta(const void* A, const void* B, void* C, int64_t M, int64_t N, int64_t K, int64_t lda,
+                              int64_t ldb, int64_t ldc, int sm_count, cudaStream_t stream, const MseEpilogue* mse) {
+  M4T_CHECK(gemm_bf16_tn_supported(M, N, K, A, B, C, lda, ldb, ldc), "unsupported GEMM shape/alignment for the wgmma path");
+  constexpr int BN = tile_n<false>();
+  const CUtensorMap ta = make_tmap(A, M, K, lda, BM);
+  const CUtensorMap tb = make_tmap(B, N, K, ldb, BN / 2);  // each CTA of the pair loads half of the B tile
+  GemmArgs g{};
+  g.C = C;
+  g.M = static_cast<int>(M);
+  g.N = static_cast<int>(N);
+  g.K = static_cast<int>(K);
+  g.ldc = static_cast<int>(ldc);
+  const int tiles = static_cast<int>(((M + 2 * BM - 1) / (2 * BM)) * ((N + BN - 1) / BN));
+  const int pairs = std::max(1, std::min(tiles, sm_count / 2));
+  if (mse) {
+    set_mse(g, mse);
+    launch_pair<1>(pairs, ta, tb, g, stream, "gemm_2cta_mse_epilogue");
+  } else {
+    launch_pair<0>(pairs, ta, tb, g, stream, "gemm_2cta");
+  }
+}
+
+bool gemm_bf16_nn_supported(int64_t M, int64_t N, int64_t K, const void* A, const void* B, const void* C, int64_t lda,
+                            int64_t ldb, int64_t ldc) {
+  auto al = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
+  return M > 0 && N > 0 && K > 0 && N % 8 == 0 && K % 8 == 0 && al(A) && al(B) && al(C) && lda % 8 == 0 && ldb % 8 == 0 &&
+         ldc % 8 == 0 && lda >= K && ldb >= N && ldc >= N && M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31);
+}
+
+// C[M,N] = A[M,K] * B[K,N], both row-major (the dgrad shape: gy @ W).
+void launch_gemm_bf16_nn(const void* A, const void* B, void* C, int64_t M, int64_t N, int64_t K, int64_t lda,
+                         int64_t ldb, int64_t ldc, int sm_count, cudaStream_t stream) {
+  M4T_CHECK(gemm_bf16_nn_supported(M, N, K, A, B, C, lda, ldb, ldc), "unsupported GEMM shape/alignment for the wgmma NN path");
+  constexpr int BN = tile_n<false>();
+  const CUtensorMap ta = make_tmap(A, M, K, lda, BM);
+  const CUtensorMap tb = make_tmap_bf16_sw128(B, K, N, ldb, 64, BK);  // boxes of {64 n, BK k-rows}
+  GemmArgs g{};
+  g.C = C;
+  g.M = static_cast<int>(M);
+  g.N = static_cast<int>(N);
+  g.K = static_cast<int>(K);
+  g.ldc = static_cast<int>(ldc);
+  const int tiles = static_cast<int>(((M + BM - 1) / BM) * ((N + BN - 1) / BN));
+  const int grid = std::max(1, std::min(tiles, sm_count));
+  launch<false, 0, true>(grid, ta, tb, g, CommArgs{}, stream, "gemm_nn");
+}
+
+// y = x @ mean_ranks(W)^T in ONE kernel.  `w_off`/`wavg_off`/`flags_off` are
+// byte offsets inside the symmetric heap (identical on all ranks); the weight
+// must already be staged at w_off on every rank.
+void launch_fused_allreduce_gemm(const DeviceComm& dc, const void* x, void* y, int64_t M, int64_t N, int64_t K,
+                                 int64_t ldx, int64_t ldy, int64_t w_off, int64_t wavg_off, int64_t flags_off,
+                                 uint32_t panel_target, float scale, cudaStream_t stream, const MseEpilogue* mse) {
+  M4T_CHECK(dc.mc_heap != nullptr, "the fused Allreduce->GEMM kernel needs the NVLS multicast mapping");
+  const int P = dc.sync.size;
+  M4T_CHECK(kPanel % P == 0 && N % kPanel == 0 && (K * 2) % 16 == 0,
+            "fused Allreduce->GEMM: N must be a multiple of 256 and 256 % ranks == 0");
+  const char* wavg = dc.heap[dc.sync.rank] + wavg_off;
+  M4T_CHECK(gemm_bf16_tn_supported(M, N, K, x, wavg, y, ldx, K, ldy), "unsupported GEMM shape/alignment for the fused path");
+  constexpr int BN = tile_n<true>();
+  const CUtensorMap ta = make_tmap(x, M, K, ldx, BM);
+  const CUtensorMap tb = make_tmap(wavg, N, K, K, BN);
+  GemmArgs g{};
+  g.C = y;
+  g.M = static_cast<int>(M);
+  g.N = static_cast<int>(N);
+  g.K = static_cast<int>(K);
+  g.ldc = static_cast<int>(ldy);
+  g.panel_flags = reinterpret_cast<const uint32_t*>(dc.heap[dc.sync.rank] + flags_off);
+  g.panel_target = panel_target;
+  CommArgs cm{};
+  cm.sync = dc.sync;
+  cm.mc_heap = dc.mc_heap;
+  cm.my_heap = dc.heap[dc.sync.rank];
+  cm.w_off = w_off;
+  cm.wavg_off = wavg_off;
+  cm.flags_off = flags_off;
+  cm.scale = scale;
+  cm.do_barrier = 1;
+  static const int fused_debug = static_cast<int>(env_i64("M4T_FUSED_DEBUG", 0));  // read once
+  cm.debug_skip = fused_debug;
+  if (cm.debug_skip & 2) g.M = 0;  // timing experiment: communication only, no GEMM tiles
+  // the grid must be identical on every rank (per-block barrier + counter targets)
+  const int grid = fused_gemm_grid(dc);
+  if (mse) {
+    set_mse(g, mse);
+    launch<true, 1, false>(grid, ta, tb, g, cm, stream, "fused_allreduce_gemm_mse");
+  } else {
+    launch<true, 0, false>(grid, ta, tb, g, cm, stream, "fused_allreduce_gemm");
+  }
+}
+
+int fused_gemm_grid(const DeviceComm& dc) { return std::min(dc.sm_count, kMaxChannels) & ~1; }
+
+}  // namespace m4t

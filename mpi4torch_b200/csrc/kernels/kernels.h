@@ -1,4 +1,4 @@
-// Host-callable launchers of the sm_100a kernels.  Torch-free; the CUDA backend
+// Host-callable launchers of the sm_90a kernels.  Torch-free; the CUDA backend
 // (runtime/cuda_backend.cpp) fills a DeviceComm once and passes it by value.
 #pragma once
 #include <string>
@@ -104,7 +104,7 @@ void launch_p2p_send_ce(const SyncCtx& sync, const P2pChannel& ch, const void* s
 void launch_p2p_recv_ce(const SyncCtx& sync, const P2pChannel& ch, void* dst, int64_t bytes,
                         unsigned long long first_chunk, cudaStream_t stream);
 
-// ---- tcgen05 GEMM + fused Allreduce->GEMM (gemm_tcgen05.cu) --------------------
+// ---- wgmma GEMM + fused Allreduce->GEMM (gemm_wgmma.cu) ------------------------
 bool gemm_bf16_tn_supported(int64_t M, int64_t N, int64_t K, const void* A, const void* B, const void* C, int64_t lda,
                             int64_t ldb, int64_t ldc);
 // Optional fused MSE epilogue: instead of y the kernel stores dL/dy =
@@ -115,31 +115,27 @@ struct MseEpilogue {
   float* loss_acc;
   float loss_scale, grad_scale;
 };
-// C[M,N] = A[M,K] * B[N,K]^T, bf16 in / fp32 accumulate (TMEM) / bf16 out.
+// C[M,N] = A[M,K] * B[N,K]^T, bf16 in / fp32 accumulate / bf16 out.
 void launch_gemm_bf16_tn(const void* A, const void* B, void* C, int64_t M, int64_t N, int64_t K, int64_t lda,
                          int64_t ldb, int64_t ldc, int sm_count, cudaStream_t stream, const MseEpilogue* mse = nullptr);
-// Same contract on CTA pairs (cta_group::2, 256x256 cluster tiles, 6-stage TMA ring).
+// Same contract on CTA pairs (clusters of two, 256x256 tiles, B tile multicast to both CTAs).
 void launch_gemm_bf16_tn_2cta(const void* A, const void* B, void* C, int64_t M, int64_t N, int64_t K, int64_t lda,
                               int64_t ldb, int64_t ldc, int sm_count, cudaStream_t stream, const MseEpilogue* mse = nullptr);
 // y = x @ (scale * sum_ranks W)^T in one kernel; W staged at heap offset w_off on every rank.
 void launch_fused_allreduce_gemm(const DeviceComm& dc, const void* x, void* y, int64_t M, int64_t N, int64_t K,
                                  int64_t ldx, int64_t ldy, int64_t w_off, int64_t wavg_off, int64_t flags_off,
                                  uint32_t panel_target, float scale, cudaStream_t stream, const MseEpilogue* mse = nullptr);
-void launch_fused_allreduce_gemm_2cta(const DeviceComm& dc, const void* x, void* y, int64_t M, int64_t N, int64_t K,
-                                      int64_t ldx, int64_t ldy, int64_t w_off, int64_t wavg_off, int64_t flags_off,
-                                      uint32_t panel_target, float scale, cudaStream_t stream,
-                                      const MseEpilogue* mse = nullptr);
 int fused_gemm_grid(const DeviceComm& dc);
 
-// ---- weight gradient (wgrad_tcgen05_2cta.cu), experimental -------------------------
+// ---- weight gradient (wgrad_wgmma.cu) ------------------------------------------------
 // G[N,K] = dY[Mb,N]^T * X[Mb,K]: both operands MN-major, no transposed copies.
 bool wgrad_bf16_supported(int64_t Mb, int64_t N, int64_t K, const void* dy, const void* x, const void* g, int64_t ldy,
                           int64_t ldx, int64_t ldg);
-// C[M,N] = A[M,K] * B[K,N], both row-major bf16 (dgrad: gy @ W): the CTA-pair kernel with an MN-major B operand.
+// C[M,N] = A[M,K] * B[K,N], both row-major bf16 (dgrad: gy @ W): the wgmma kernel with an MN-major B operand.
 bool gemm_bf16_nn_supported(int64_t M, int64_t N, int64_t K, const void* A, const void* B, const void* C, int64_t lda,
                             int64_t ldb, int64_t ldc);
-void launch_gemm_bf16_nn_2cta(const void* A, const void* B, void* C, int64_t M, int64_t N, int64_t K, int64_t lda,
-                              int64_t ldb, int64_t ldc, int sm_count, cudaStream_t stream);
+void launch_gemm_bf16_nn(const void* A, const void* B, void* C, int64_t M, int64_t N, int64_t K, int64_t lda,
+                         int64_t ldb, int64_t ldc, int sm_count, cudaStream_t stream);
 void launch_wgrad_bf16(const void* dy, const void* x, void* g, int64_t Mb, int64_t N, int64_t K, int64_t ldy,
                        int64_t ldx, int64_t ldg, int sm_count, cudaStream_t stream, const float* gscale = nullptr,
                        float axpy = 0.0f);

@@ -1,0 +1,147 @@
+// Shared main loop of the Hopper GEMM kernels (gemm_wgmma.cu, wgrad_wgmma.cu).
+//
+// One persistent CTA per SM computes 128 x BN output tiles (BN = 256, or 128 for the fused
+// kernels, whose communication warps need the registers) with BK = 64:
+//   warpgroup 0 (warp 0, one lane)  TMA producer: A/B tiles -> smem ring of Tile<BN>::kStages
+//   warpgroups 1, 2                 consumers: 64 rows each, wgmma m64nBNk16 into BN/2 fp32
+//                                   registers per thread, epilogue straight from registers
+//   further warps                   (fused kernels only) communication role
+// CL = 2 runs the same loop on a cluster of two CTAs that share one 256 x BN tile: each CTA
+// stages its own 128 rows of A and loads HALF of the B tile, multicast by TMA into both CTAs,
+// so a pair moves 2/3 of the L2 -> SMEM bytes of two independent CTAs.  A stage may only be
+// refilled when the consumers of BOTH CTAs released it: the empty barriers count both.
+// Each operand is either K-major (one TMA box {64 k, rows}) or MN-major (boxes of
+// {64 contiguous m/n, 64 k-rows}); the wgmma transpose bits select the layout, so no
+// operand is ever copied transposed.
+#pragma once
+#include "hopper_ptx.cuh"
+#include "vec_ops.cuh"
+
+namespace m4t {
+namespace wg {
+
+constexpr int BM = 128, BK = 64;
+constexpr int kBoxBytesMN = 64 * BK * 2;  // 8 KiB: one MN-major box
+constexpr int kABytes = BM * BK * 2;      // 16 KiB
+constexpr int kGemmThreads = 384;         // producer warpgroup + two consumer warpgroups
+constexpr int kConsumerWarps = 8;
+constexpr int kMaxStages = 6;
+
+template <int BN> struct Tile {
+  static_assert(BN == 128 || BN == 256, "tile width");
+  static constexpr int kBBytes = BN * BK * 2;
+  static constexpr int kStageBytes = kABytes + kBBytes;
+  static constexpr int kStages = BN == 256 ? 4 : kMaxStages;  // ~192 KiB of ring either way
+  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align*/ + 256 /*barriers*/;
+};
+
+struct __align__(8) Pipe {
+  uint64_t full[kMaxStages];
+  uint64_t empty[kMaxStages];
+};
+
+__device__ __forceinline__ uint8_t* aligned_smem(uint8_t* raw) {
+  return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw) + 1023) & ~uintptr_t(1023));
+}
+template <int BN> __device__ __forceinline__ Pipe* pipe_of(uint8_t* smem) {
+  return reinterpret_cast<Pipe*>(smem + Tile<BN>::kStages * Tile<BN>::kStageBytes);
+}
+
+template <int BN, int CL = 1> __device__ __forceinline__ void init_pipe(Pipe* p) {
+  for (int s = 0; s < Tile<BN>::kStages; ++s) {
+    tc::mbar_init(&p->full[s], 1);
+    tc::mbar_init(&p->empty[s], kConsumerWarps * CL);  // one arrive per consumer warp of every CTA that writes here
+  }
+  tc::fence_barrier_init();
+}
+
+template <int BN> __device__ __forceinline__ void advance(int& stage, uint32_t& phase) {
+  if (++stage == Tile<BN>::kStages) {
+    stage = 0;
+    phase ^= 1;
+  }
+}
+
+// Producer: one stage = A rows [m0, m0+128) and B rows [n0, n0+BN) of the k-slice starting at k0.
+// CL = 2: this CTA (cluster rank `crank`) loads B rows [n0 + crank*BN/2, +BN/2) into both CTAs.
+template <bool A_MN, bool B_MN, int BN, int CL = 1>
+__device__ __forceinline__ void load_stage(uint8_t* smem, Pipe* p, int& stage, uint32_t& phase, const CUtensorMap* ma,
+                                           const CUtensorMap* mb, int m0, int n0, int k0, uint32_t crank = 0) {
+  static_assert(CL == 1 || !B_MN, "the CTA pair splits a K-major B tile");
+  tc::mbar_wait(&p->empty[stage], phase ^ 1);
+  uint8_t* sa = smem + stage * Tile<BN>::kStageBytes;
+  uint8_t* sb = sa + kABytes;
+  tc::mbar_arrive_expect_tx(&p->full[stage], Tile<BN>::kStageBytes);
+  if (A_MN) {
+#pragma unroll
+    for (int ch = 0; ch < BM / 64; ++ch) tc::tma_load_2d(sa + ch * kBoxBytesMN, ma, &p->full[stage], m0 + ch * 64, k0);
+  } else {
+    tc::tma_load_2d(sa, ma, &p->full[stage], k0, m0);
+  }
+  if (CL == 2) {
+    const int half = static_cast<int>(crank) * (BN / 2);
+    tc::tma_load_2d_multicast(sb + half * 128, mb, &p->full[stage], k0, n0 + half, 0x3);
+  } else if (B_MN) {
+#pragma unroll
+    for (int ch = 0; ch < BN / 64; ++ch) tc::tma_load_2d(sb + ch * kBoxBytesMN, mb, &p->full[stage], n0 + ch * 64, k0);
+  } else {
+    tc::tma_load_2d(sb, mb, &p->full[stage], k0, n0);
+  }
+  advance<BN>(stage, phase);
+}
+
+// Consumer warpgroup `wgi` (0/1): acc = its 64 rows of the tile, summed over k_blocks stages.
+// The stage of k-block kb is handed back to the producer once the wgmma of kb + 1 has been
+// issued and those of kb have retired (wait_group 1), so one k-block of MMAs is always queued.
+template <bool A_MN, bool B_MN, int BN, int CL = 1>
+__device__ __forceinline__ void mma_tile(float (&acc)[BN / 2], uint8_t* smem, Pipe* p, int& stage, uint32_t& phase,
+                                         int k_blocks, int wgi, uint32_t crank = 0) {
+  const int lane = threadIdx.x & 31;
+  // the stage is free again for every producer that wrote into it: this CTA's and, in a pair, the peer's
+  auto release = [&](int s) {
+    if (lane != 0) return;
+    tc::mbar_arrive(&p->empty[s]);
+    if (CL == 2) tc::mbar_arrive_remote(&p->empty[s], crank ^ 1u);
+  };
+  int prev = -1;
+  tc::fence_regs(acc);
+  for (int kb = 0; kb < k_blocks; ++kb) {
+    tc::mbar_wait(&p->full[stage], phase);
+    const uint32_t sa = tc::smem_u32(smem + stage * Tile<BN>::kStageBytes);
+    const uint32_t sb = sa + kABytes;
+    // this warpgroup's 64 rows of A: one MN-major box, or 64 K-major rows of 128 bytes
+    const uint32_t a0 = sa + static_cast<uint32_t>(wgi) * (A_MN ? kBoxBytesMN : 64 * 128);
+    tc::wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k) {
+      // next 16 k: 32 bytes along a K-major row, or two 8-row atoms (2048 bytes) of an MN-major box
+      const uint64_t da = tc::make_desc_sw128(a0 + (A_MN ? k * 2048 : k * 32), A_MN ? kBoxBytesMN : 16);
+      const uint64_t db = tc::make_desc_sw128(sb + (B_MN ? k * 2048 : k * 32), B_MN ? kBoxBytesMN : 16);
+      if constexpr (BN == 256)
+        tc::wgmma_m64n256k16_bf16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, (kb | k) ? 1u : 0u);
+      else
+        tc::wgmma_m64n128k16_bf16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, (kb | k) ? 1u : 0u);
+    }
+    tc::wgmma_commit();
+    tc::wgmma_wait<1>();
+    if (prev >= 0) release(prev);
+    prev = stage;
+    advance<BN>(stage, phase);
+  }
+  tc::wgmma_wait<0>();
+  tc::fence_regs(acc);
+  if (prev >= 0) release(prev);
+}
+
+// Accumulator fragment of wgmma m64nN (fp32): thread (warp w of the warpgroup, lane l) holds, for
+// j = 0 .. N/8 - 1, columns 8j + 2(l % 4) + {0, 1} of rows 16w + l / 4 (acc[4j], acc[4j+1]) and
+// 16w + l / 4 + 8 (acc[4j+2], acc[4j+3]).
+__device__ __forceinline__ int frag_row(int h) { return ((threadIdx.x >> 5) & 3) * 16 + ((threadIdx.x & 31) >> 2) + 8 * h; }
+__device__ __forceinline__ int frag_col(int j) { return 8 * j + 2 * (threadIdx.x & 3); }
+
+__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
+  return static_cast<uint32_t>(float_to_bf16_bits(lo)) | (static_cast<uint32_t>(float_to_bf16_bits(hi)) << 16);
+}
+
+}  // namespace wg
+}  // namespace m4t

@@ -2,8 +2,8 @@
 //   * CpuBackend  - POSIX shared memory + atomics (plumbing, local tests, the
 //                   host-staged comparator; reference analogue: plain MPI on host
 //                   buffers, csrc/extension.cpp:61-104),
-//   * CudaBackend - symmetric heap over NVLink 5 / NVSwitch with hand-written
-//                   sm_100a kernels (the product).
+//   * CudaBackend - symmetric heap over NVLink 4 / NVSwitch with hand-written
+//                   sm_90a kernels (the product).
 // All pointers are raw; `stream` is an opaque cudaStream_t for the CUDA backend
 // and ignored by the CPU backend (whose calls are host-blocking like MPI).
 #pragma once

@@ -28,7 +28,7 @@ CudaBackend::CudaBackend(Control& ctl, int device, int64_t stage_mb, int64_t sym
   tune_.chunk_bytes = env_i64("M4T_CHUNK_KB", 0) * 1024;
   tune_.pipe_min_bytes = env_i64("M4T_PIPE_MIN_MB", 512) << 20;
   tune_.nvls_min_ranks = static_cast<int>(env_i64("M4T_NVLS_MIN_RANKS", 4));
-  tune_.ar_blocks = static_cast<int>(env_i64("M4T_AR_BLOCKS", 148));
+  tune_.ar_blocks = static_cast<int>(env_i64("M4T_AR_BLOCKS", 132));
   tune_.oneshot_blocks = static_cast<int>(env_i64("M4T_ONESHOT_BLOCKS", 32));
   tune_.slab_blocks = static_cast<int>(env_i64("M4T_SLAB_BLOCKS", 128));
   tune_.p2p_blocks = static_cast<int>(env_i64("M4T_P2P_BLOCKS", 32));
@@ -353,14 +353,7 @@ bool CudaBackend::fused_linear_available(int64_t N, int64_t K) const {
 void CudaBackend::gemm_bf16_tn(const void* A, const void* B, void* C, int64_t M, int64_t N, int64_t K, int64_t lda,
                                int64_t ldb, int64_t ldc, cudaStream_t stream, const MseEpilogue* mse) {
   M4T_CUDA(cudaSetDevice(device_));
-  // CTA-pair kernel for anything big enough to fill the pairs; M4T_GEMM_2CTA=0/1 forces.
-  static const int64_t mode = env_i64("M4T_GEMM_2CTA", -1);
-  const bool big = M >= 512 && N >= 512;
-  if (mode == 1 || (mode < 0 && big && gemm_2cta_default_)) {
-    launch_gemm_bf16_tn_2cta(A, B, C, M, N, K, lda, ldb, ldc, dc_.sm_count, stream, mse);
-  } else {
-    launch_gemm_bf16_tn(A, B, C, M, N, K, lda, ldb, ldc, dc_.sm_count, stream, mse);
-  }
+  launch_gemm_bf16_tn(A, B, C, M, N, K, lda, ldb, ldc, dc_.sm_count, stream, mse);
 }
 
 const void* CudaBackend::fused_allreduce_linear(const void* x, const void* w, void* y, int64_t M, int64_t N, int64_t K,
@@ -395,14 +388,8 @@ const void* CudaBackend::fused_allreduce_linear(const void* x, const void* w, vo
   const int par = static_cast<int>(st.calls & 1);
   st.calls += 1;
   const uint32_t target = static_cast<uint32_t>(st.calls * static_cast<uint64_t>(size()) * fused_gemm_grid(dc_));
-  static const int64_t fused_2cta = env_i64("M4T_FUSED_2CTA", 1);
-  if (fused_2cta) {
-    launch_fused_allreduce_gemm_2cta(dc_, x, y, M, N, K, ldx, ldy, w_off, st.wavg_off[par], st.flags_off, target,
-                                     scale, stream, mse);
-  } else {
-    launch_fused_allreduce_gemm(dc_, x, y, M, N, K, ldx, ldy, w_off, st.wavg_off[par], st.flags_off, target, scale,
-                                stream, mse);
-  }
+  launch_fused_allreduce_gemm(dc_, x, y, M, N, K, ldx, ldy, w_off, st.wavg_off[par], st.flags_off, target, scale,
+                              stream, mse);
   return symm_ptr(st.wavg_off[par]);
 }
 
@@ -434,10 +421,10 @@ const void* CudaBackend::fused_wgrad_update(void* w, const void* dy, const void*
   auto it = wgrad_.find(key);
   if (it == wgrad_.end()) {
     FusedWgradState st;
-    // two work units per tile even out the last wave on 74 CTA pairs (M4T_WGRAD_KSPLIT=1 disables)
+    // two work units per tile even out the last wave of the CTAs (M4T_WGRAD_KSPLIT=1 disables)
     static const int64_t ksplit_env = env_i64("M4T_WGRAD_KSPLIT", 2);  // read once
     st.ksplit = (ksplit_env >= 2 && (Mb / 64) % 2 == 0) ? 2 : 1;
-    st.stage_stride = N * K * 2;  // dense: the peer-store epilogue addresses [ksplit * N, K] through one tensor map
+    st.stage_stride = N * K * 2;  // dense: the peer-store epilogue addresses [ksplit * N, K] rows of the owner's area
     // multicast mode: one staging area per rank (own partials, pulled through the switch by the owners);
     // peer-store mode: one area per SOURCE rank in every heap (the epilogues push to the owner)
     st.src_stride = st.stage_stride * st.ksplit;

@@ -160,7 +160,6 @@ class CudaBackend final : public Backend {
   std::unordered_map<int64_t, FusedWgradState> wgrad_;  // key = N << 32 | K
   int64_t symm_off_ = 0, symm_cursor_ = 0, symm_bytes_ = 0;
   int64_t p2p_ce_min_bytes_ = 2 << 20;  // copy-engine path threshold (M4T_P2P_CE_MIN_KB)
-  bool gemm_2cta_default_ = true;  // CTA-pair kernel validated on B200: 1521 vs 1390 TFLOP/s (cuBLAS 1552)
 };
 
 }  // namespace m4t

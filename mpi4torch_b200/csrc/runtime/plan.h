@@ -1,4 +1,4 @@
-// Slab plans: the B200-native replacement for the reference's MPI derived
+// Slab plans: the H100-native replacement for the reference's MPI derived
 // datatypes (MPI_Type_vector + create_resized, duplicated at reference
 // csrc/extension.cpp:516-591, :651-726, :788-876).
 //
@@ -7,7 +7,7 @@
 // pulls out of peers' staged inputs.  A box is up to three outer loops around a
 // contiguous run, all in 64-bit element units (no INT_MAX limits, cf.
 // reference :530, :665, :810).  The same plan drives the CPU shared-memory
-// backend (memcpy) and the sm_100a slab kernels (peer loads over NVLink).
+// backend (memcpy) and the sm_90a slab kernels (peer loads over NVLink).
 #pragma once
 #include <cstdint>
 #include <vector>

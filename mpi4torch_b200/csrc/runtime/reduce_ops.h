@@ -1,5 +1,5 @@
 // Element types and reduction functors shared by the CPU shared-memory backend
-// (g++) and the sm_100a kernels (nvcc).  Everything is header-only and
+// (g++) and the sm_90a kernels (nvcc).  Everything is header-only and
 // host/device clean.
 //
 // Covers the reference's 12-op table (csrc/extension.cpp:204-252) over the

@@ -34,7 +34,7 @@ KNOBS: Dict[str, Tuple[str, str]] = {
     "M4T_ALLREDUCE_ALGO": ("0", "force an algorithm: 1 one-shot, 2 two-shot (peer loads), 3 NVLS; 0 = by size"),
     "M4T_ONESHOT_MAX_KB": ("2048", "largest message of the one-shot algorithm"),
     "M4T_ONESHOT_BLOCKS": ("32", "CTAs of the one-shot kernel"),
-    "M4T_AR_BLOCKS": ("148", "CTAs of the two-shot / NVLS kernels"),
+    "M4T_AR_BLOCKS": ("132", "CTAs of the two-shot / NVLS kernels"),
     "M4T_AR_PIPE": ("1", "0 disables the pipelined NVLS kernel for large messages"),
     "M4T_PIPE_MIN_MB": ("512", "smallest message of the pipelined NVLS kernel"),
     "M4T_CHUNK_KB": ("0", "cap on the bytes one allreduce launch moves (0 = half a staging half)"),
@@ -48,12 +48,9 @@ KNOBS: Dict[str, Tuple[str, str]] = {
     "M4T_P2P_PUSH": ("0", "1 places each pair's ring in the receiver's heap (sender pushes)"),
     "M4T_P2P_CE_MIN_KB": ("2048", "messages from this size move on the copy engines; negative = never"),
     # ---- tensor-core kernels
-    "M4T_GEMM_2CTA": ("-1", "1 / 0 force / forbid the CTA-pair GEMM; -1 = by shape"),
     "M4T_FUSED_LINEAR": ("1", "0 disables the fused Allreduce->GEMM forward"),
-    "M4T_FUSED_2CTA": ("1", "0 runs the fused forward on the single-CTA kernel"),
     "M4T_FUSED_WGRAD": ("1", "0 disables the fused backward (wgrad -> reduce-scatter -> SGD -> multicast)"),
     "M4T_WGRAD_KSPLIT": ("2", "batch split of the last partial wave of the fused backward"),
-    "M4T_EPI_PREFETCH": ("0", "1 prefetches the target tile in the GEMM+MSE epilogue"),
     "M4T_WGRAD_DEBUG": ("0", "timing experiments: bit mask of fused-backward phases to skip (wrong results)"),
     "M4T_FUSED_DEBUG": ("0", "timing experiments: bit mask of fused-forward phases to skip (wrong results)"),
     # ---- waits, diagnostics
@@ -96,7 +93,7 @@ def build_facts() -> Dict[str, object]:
         "extension": str(so),
         "extension_exists": so.exists(),
         "extension_fresh": bool(so.exists() and _build.is_fresh()),
-        "target": "sm_100a (compute_100a), no other architecture is built",
+        "target": "sm_90a (compute_90a), no other architecture is built",
         "cuda_visible": bool(torch.cuda.is_available()),
         "gpus": torch.cuda.device_count() if torch.cuda.is_available() else 0,
     }

@@ -1,4 +1,4 @@
-"""Data-parallel linear layer as autograd nodes backed by the fused tcgen05 kernels.
+"""Data-parallel linear layer as autograd nodes backed by the fused wgmma kernels.
 
 ``allreduce_linear(x, W)``         y = x @ mean_ranks(W)^T
 ``dp_linear_mse(x, W, t, ...)``    loss_local = loss_scale * sum((x @ mean_ranks(W)^T - t)^2)
@@ -7,9 +7,9 @@ Both are ``torch.autograd.Function`` nodes (the reference builds its nodes the s
 csrc/extension.cpp:254-308: forward communicates, backward runs the adjoint communication):
 
 * forward  = ONE kernel: the parameter Allreduce (x 1/size) fused into the GEMM operand path
-  (csrc/kernels/gemm_tcgen05_2cta.cu, ``FUSED``), for ``dp_linear_mse`` with the loss and dL/dy
+  (csrc/kernels/gemm_wgmma.cu, ``FUSED``), for ``dp_linear_mse`` with the loss and dL/dy
   produced by the GEMM epilogue;
-* backward = the weight-gradient GEMM (csrc/kernels/wgrad_tcgen05_2cta.cu, MN-major tcgen05) and
+* backward = the weight-gradient GEMM (csrc/kernels/wgrad_wgmma.cu, MN-major wgmma operands) and
   the adjoint Allreduce of the gradient.  With an :class:`InBackwardSGD` attached, backward is ONE
   kernel: wgrad GEMM -> reduce-scatter through the NVSwitch -> ``W += -lr/size * sum`` -> multicast of
   the new weights (-> Allreduce of the new weights for the next forward), i.e. the optimizer step runs
@@ -83,7 +83,7 @@ def _wgrad(gy: torch.Tensor, x: torch.Tensor, gscale: Optional[torch.Tensor] = N
 
 
 def _dgrad(gy: torch.Tensor, w: torch.Tensor) -> torch.Tensor:
-    """gy @ w on the library's own kernel when it applies (mixed-major tcgen05 GEMM)."""
+    """gy @ w on the library's own kernel when it applies (mixed-major wgmma GEMM)."""
     if gy.is_cuda and gy.dim() == 2 and gy.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 \
             and m4t.cuda_backend_ready() and hasattr(_ops(), "gemm_bf16_nn") and _ops().gemm_bf16_nn_supported(gy, w):
         return _ops().gemm_bf16_nn(gy, w)

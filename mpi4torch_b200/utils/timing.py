@@ -1,6 +1,6 @@
 """Measurement hygiene shared by bench.py and the sweep scripts.
 
-Rules (B200_PROFILING.md): time on the device with CUDA events on the launching
+Rules: time on the device with CUDA events on the launching
 stream, >= 3 warm-ups, flush L2 between timed iterations (or use inputs larger
 than L2), take the max over ranks, and sample SM clocks / throttle reasons
 DURING the timed region.
@@ -17,7 +17,7 @@ import torch
 
 
 class L2Flusher:
-    """Writes a buffer larger than the 126 MB L2 so the next iteration starts cold."""
+    """Writes a buffer larger than the 50 MB L2 so the next iteration starts cold."""
 
     def __init__(self, device, nbytes: int = 256 << 20):
         self.buf = torch.empty(nbytes, dtype=torch.uint8, device=device)

@@ -1,4 +1,4 @@
-"""Packaging: the native core is compiled in-tree for sm_100a (see
+"""Packaging: the native core is compiled in-tree for sm_90a (see
 mpi4torch_b200/_build.py); ``pip install .`` builds it once at install time.
 
 The reference drives its single C++ TU through ``mpicc``/``mpicxx`` (reference

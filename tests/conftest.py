@@ -15,7 +15,7 @@ sys.path.insert(0, str(ROOT))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs at least one CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs at least one CUDA device (run on an H100 box)")
 
 
 def run_spmd(nprocs, script_args, *, device="cpu", timeout=600, extra_env=None):

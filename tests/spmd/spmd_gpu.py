@@ -229,7 +229,7 @@ class TestFusedAllreduceLinear(unittest.TestCase):
         scale = w2.grad.float().abs().max().item() + 1e-6
         self.assertLess((w1.grad.float() - w2.grad.float()).abs().max().item() / scale, 5e-2)
 
-    def test_tcgen05_gemm_inside_spmd(self):
+    def test_wgmma_gemm_inside_spmd(self):
         x = torch.randn(300, 192, generator=torch.Generator().manual_seed(1)).to(torch.bfloat16).to(DEVICE)
         w = torch.randn(520, 192, generator=torch.Generator().manual_seed(2)).to(torch.bfloat16).to(DEVICE)
         y = torch.ops.mpi4torch_b200.gemm_bf16_tn(x, w)

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM numerics against a plain fp32 PyTorch reference."""
+"""wgmma GEMM numerics against a plain fp32 PyTorch reference."""
 import pytest
 import torch
 
@@ -55,7 +55,7 @@ def test_gemm_speed_report():
     M, N, K = 8192, 4096, 4096
     x = torch.randn(M, K, device="cuda").to(torch.bfloat16)
     w = torch.randn(N, K, device="cuda").to(torch.bfloat16)
-    for name, fn in (("tcgen05", lambda: torch.ops.mpi4torch_b200.gemm_bf16_tn(x, w)), ("cublas", lambda: x @ w.t())):
+    for name, fn in (("wgmma", lambda: torch.ops.mpi4torch_b200.gemm_bf16_tn(x, w)), ("cublas", lambda: x @ w.t())):
         for _ in range(3):
             fn()
         torch.cuda.synchronize()
@@ -102,10 +102,11 @@ def test_gemm_2cta_speed_report():
     b.record()
     b.synchronize()
     ms = a.elapsed_time(b) / 10
-    print(f"[gemm] tcgen05 cta_group::2: {ms:.3f} ms  {2.0 * M * N * K / ms / 1e9:.1f} TFLOP/s")
+    print(f"[gemm] wgmma CTA pair: {ms:.3f} ms  {2.0 * M * N * K / ms / 1e9:.1f} TFLOP/s")
 
 
-@pytest.mark.parametrize("shape", [(64, 256, 256), (128, 256, 512), (512, 512, 256), (8192, 4096, 4096), (4096, 1024, 2048)])
+@pytest.mark.parametrize("shape", [(64, 256, 256), (128, 256, 512), (512, 512, 256), (8192, 4096, 4096), (4096, 1024, 2048),
+                                   (256, 384, 640)])
 def test_wgrad_mn_major_matches_fp32_reference(shape):
     import mpi4torch_b200 as m4t  # noqa: F401
 
@@ -130,8 +131,8 @@ def test_wgrad_mn_major_matches_fp32_reference(shape):
 @pytest.mark.parametrize("shape", [(256, 256, 64), (384, 512, 256), (8192, 4096, 4096), (300, 520, 200), (1000, 1000, 1000),
                                    (130, 264, 72)])
 def test_linear_mse_epilogue_matches_fp32_reference(shape):
-    """GEMM with the fused loss epilogue (dL/dy = g * (x W^T - t), loss = s * sum((x W^T - t)^2)); both the
-    CTA-pair kernel (large shapes) and the single-CTA kernel (small ones), including ragged tiles."""
+    """GEMM with the fused loss epilogue (dL/dy = g * (x W^T - t), loss = s * sum((x W^T - t)^2)), large
+    shapes and ragged tiles."""
     import mpi4torch_b200 as m4t  # noqa: F401
 
     m4t.COMM_WORLD
@@ -158,7 +159,7 @@ def test_linear_mse_epilogue_matches_fp32_reference(shape):
 
 @pytest.mark.parametrize("shape", [(256, 256, 64), (512, 768, 256), (8192, 4096, 4096), (300, 520, 200), (1000, 1000, 1000)])
 def test_gemm_nn_dgrad_matches_fp32_reference(shape):
-    """gy[M,N] @ W[N,K] with the weight read in place as an MN-major tcgen05 operand (no transposed copy)."""
+    """gy[M,N] @ W[N,K] with the weight read in place as an MN-major wgmma operand (no transposed copy)."""
     import mpi4torch_b200 as m4t  # noqa: F401
 
     m4t.COMM_WORLD

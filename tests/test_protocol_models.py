@@ -1,5 +1,5 @@
 """Pure-Python mirrors of the index arithmetic of the fused backward kernel
-(csrc/kernels/wgrad_tcgen05_2cta.cu).  They cannot check the memory model, but they do
+(csrc/kernels/wgrad_wgmma.cu).  They cannot check the memory model, but they do
 check what is easy to get wrong in a persistent, role-split kernel: that the work
 distribution covers every element exactly once and that the counters reach exactly the
 targets the host computes (csrc/runtime/cuda_backend.cpp::fused_wgrad_update)."""
@@ -8,20 +8,21 @@ import itertools
 import numpy as np
 import pytest
 
-BMC, BM2, BN = 128, 256, 256          # rows per CTA, rows / cols per cluster tile
-K_COMM_WARPS, K_U, K_ROW_SPLIT = 8, 4, 2
-K_ROWS = BMC // K_ROW_SPLIT
-SIGNALS_PER_UNIT = 8                  # 4 epilogue warps x 2 CTAs
+BM, BN = 128, 128                     # rows / cols of a tile of G (one CTA)
+K_COMM_WARPS, K_U, K_ROW_SPLIT = 4, 4, 2
+K_PAIRS = BM // K_ROW_SPLIT // 2      # row pairs of one owner work item (half a warp per 256-byte row)
+SIGNALS_PER_UNIT = 8                  # 2 consumer warpgroups x 4 warps
+WARP_ROWS = 16                        # rows of the wgmma accumulator fragment held by one warp
 
 
-def units_of_cluster(cluster_id, num_clusters, num_units):
-    return range(cluster_id, num_units, num_clusters)
+def units_of_cta(cta, num_ctas, num_units):
+    return range(cta, num_units, num_ctas)
 
 
-def make_sched(num_tiles, num_clusters, ksplit):
+def make_sched(num_tiles, num_ctas, ksplit):
     """make_sched / unit_to_tile of the kernel: whole waves of tiles run over the full batch, only the tiles
     of the last partial wave are split in `ksplit` batch slices."""
-    whole = (num_tiles // num_clusters) * num_clusters if ksplit > 1 else num_tiles
+    whole = (num_tiles // num_ctas) * num_ctas if ksplit > 1 else num_tiles
     return whole, ksplit, whole + (num_tiles - whole) * ksplit
 
 
@@ -33,12 +34,12 @@ def unit_to_tile(sched, u):
     return whole + j // split, j % split, split
 
 
-@pytest.mark.parametrize("N,K,P,num_clusters,ksplit", [(1024, 512, 4, 3, 2), (512, 256, 8, 5, 2), (768, 768, 2, 7, 1),
-                                                      (4096, 4096, 8, 74, 2)])
-def test_fused_wgrad_work_distribution(N, K, P, num_clusters, ksplit):
-    n_tiles, k_tiles = N // BM2, K // BN
+@pytest.mark.parametrize("N,K,P,num_ctas,ksplit", [(1024, 512, 4, 3, 2), (512, 256, 8, 5, 2), (768, 768, 2, 7, 1),
+                                                  (4096, 4096, 8, 74, 2), (4096, 4096, 8, 132, 2)])
+def test_fused_wgrad_work_distribution(N, K, P, num_ctas, ksplit):
+    n_tiles, k_tiles = N // BM, K // BN
     num_tiles = n_tiles * k_tiles
-    sched = make_sched(num_tiles, num_clusters, ksplit)
+    sched = make_sched(num_tiles, num_ctas, ksplit)
     num_units = sched[2]
     small = N * K <= 1 << 20
 
@@ -47,35 +48,35 @@ def test_fused_wgrad_work_distribution(N, K, P, num_clusters, ksplit):
     signals = np.zeros(num_tiles, dtype=np.int64)  # per rank; the owner sums over P ranks
     parts_of = np.zeros(num_tiles, dtype=np.int64)
     kb_covered = np.zeros(num_tiles, dtype=np.int64)  # batch blocks contracted per tile (in units of 1/ksplit)
-    for cluster in range(num_clusters):
-        for u in units_of_cluster(cluster, num_clusters, num_units):
+    for cta in range(num_ctas):
+        for u in units_of_cta(cta, num_ctas, num_units):
             t, h, parts = unit_to_tile(sched, u)
             assert 0 <= t < num_tiles and 0 <= h < parts
             parts_of[t] = parts
             kb_covered[t] += ksplit // parts
             n_blk, k_blk = divmod(t, k_tiles)
-            for cta, q in itertools.product(range(2), range(4)):
+            for wgi, w in itertools.product(range(2), range(4)):
                 if small:
-                    r0 = n_blk * BM2 + cta * BMC + q * 32
-                    staged[h, r0:r0 + 32, k_blk * BN:(k_blk + 1) * BN] += 1
+                    r0 = n_blk * BM + wgi * 64 + w * WARP_ROWS
+                    staged[h, r0:r0 + WARP_ROWS, k_blk * BN:(k_blk + 1) * BN] += 1
                 signals[t] += 1
     assert (kb_covered == ksplit).all()  # every tile contracts the whole batch exactly once
     if small:
         for t in range(num_tiles):  # buffer h of tile t is written once iff the tile has a slice h
             n_blk, k_blk = divmod(t, k_tiles)
-            blk = staged[:, n_blk * BM2:(n_blk + 1) * BM2, k_blk * BN:(k_blk + 1) * BN]
+            blk = staged[:, n_blk * BM:(n_blk + 1) * BM, k_blk * BN:(k_blk + 1) * BN]
             for h in range(ksplit):
                 assert (blk[h] == (1 if h < parts_of[t] else 0)).all()
     # host: tile_target = signals_per_unit * size per call; the kernel multiplies by the tile's number of units
     assert (signals * P == SIGNALS_PER_UNIT * P * parts_of).all()
 
-    # --- owner side: every element of W updated by exactly one (rank, cluster, cta, warp, lane, trip) ---
+    # --- owner side: every element of W updated by exactly one (rank, cta, warp, lane, trip) ---
     updated = np.zeros((N, K), dtype=np.int8) if small else None
     items_total = 0
     for r in range(P):
         owned = (num_tiles - r + P - 1) // P if r < num_tiles else 0
-        for cluster in range(num_clusters):
-            for w_item in range(cluster, owned * K_ROW_SPLIT, num_clusters):
+        for cta in range(num_ctas):
+            for w_item in range(cta, owned * K_ROW_SPLIT, num_ctas):
                 j, sl = divmod(w_item, K_ROW_SPLIT)
                 t = r + j * P
                 assert t < num_tiles and t % P == r  # the epilogue signals rank t % P
@@ -83,37 +84,37 @@ def test_fused_wgrad_work_distribution(N, K, P, num_clusters, ksplit):
                 if not small:
                     continue
                 n_blk, k_blk = divmod(t, k_tiles)
-                for cta, cw in itertools.product(range(2), range(K_COMM_WARPS)):
-                    rows = []
-                    for row0 in range(cw, K_ROWS, K_COMM_WARPS * K_U):
-                        rows += [row0 + u * K_COMM_WARPS for u in range(K_U) if row0 + u * K_COMM_WARPS < K_ROWS]
-                    for row in rows:
-                        g = n_blk * BM2 + cta * BMC + sl * K_ROWS + row
-                        updated[g, k_blk * BN:(k_blk + 1) * BN] += 1  # 32 lanes x 8 bf16 = 256 columns
+                for cw in range(K_COMM_WARPS):
+                    pairs = []
+                    for pair0 in range(cw, K_PAIRS, K_COMM_WARPS * K_U):
+                        pairs += [pair0 + u * K_COMM_WARPS for u in range(K_U) if pair0 + u * K_COMM_WARPS < K_PAIRS]
+                    for pair, half in itertools.product(pairs, range(2)):  # lane >> 4 picks the row of the pair
+                        g = n_blk * BM + sl * 2 * K_PAIRS + 2 * pair + half
+                        updated[g, k_blk * BN:(k_blk + 1) * BN] += 1  # 16 lanes x 8 bf16 = 128 columns
     assert items_total == num_tiles * K_ROW_SPLIT
     if small:
         assert (updated == 1).all()
 
     # --- completion counter: every CTA of every rank reports once per call ---
-    grid = 2 * num_clusters
-    assert P * grid == P * 2 * num_clusters  # host: done_target = calls * size * fused_gemm_grid
+    grid = num_ctas
+    assert P * grid == P * num_ctas  # host: done_target = calls * size * fused_gemm_grid
 
 
 def test_unit_schedule_fills_the_last_wave():
-    # flagship shape: 256 tiles on 74 CTA pairs = 3 whole waves + 34 tiles; those are split in two batch halves
-    # (68 units <= 74 pairs), so the kernel takes 3.5 tile times instead of 4 and only 34 tiles have two partials
-    num_clusters, ksplit, num_tiles = 74, 2, 256
-    sched = make_sched(num_tiles, num_clusters, ksplit)
+    # 256 tiles on 74 CTAs = 3 whole waves + 34 tiles; those are split in two batch halves
+    # (68 units <= 74 CTAs), so the kernel takes 3.5 tile times instead of 4 and only 34 tiles have two partials
+    num_ctas, ksplit, num_tiles = 74, 2, 256
+    sched = make_sched(num_tiles, num_ctas, ksplit)
     assert sched == (222, 2, 290)
-    cost = [0.0] * num_clusters
-    for cluster in range(num_clusters):
-        for u in units_of_cluster(cluster, num_clusters, sched[2]):
-            cost[cluster] += 1.0 / unit_to_tile(sched, u)[2]
+    cost = [0.0] * num_ctas
+    for cta in range(num_ctas):
+        for u in units_of_cta(cta, num_ctas, sched[2]):
+            cost[cta] += 1.0 / unit_to_tile(sched, u)[2]
     assert max(cost) == 3.5
-    # both halves of a split tile run in the same (last) wave on neighbouring pairs
+    # both halves of a split tile run in the same (last) wave on neighbouring CTAs
     for t in range(sched[0], num_tiles):
         u0 = sched[0] + 2 * (t - sched[0])
-        assert u0 // num_clusters == (u0 + 1) // num_clusters == 3
+        assert u0 // num_ctas == (u0 + 1) // num_ctas == 3
 
 
 def _swizzle128(byte_off: int) -> int:
@@ -123,14 +124,14 @@ def _swizzle128(byte_off: int) -> int:
 
 def test_mn_major_descriptor_addresses_what_tma_wrote():
     """wgrad operand tile: TMA boxes of {64 contiguous elements, BK rows} with SWIZZLE_128B, read by
-    tcgen05.mma through an MN-major SWIZZLE_128B descriptor with LBO = one box, SBO = 1024 B and a
-    start-address advance of 2048 B per UMMA_K = 16 (make_smem_desc_mn_sw128, MMA issue loop).
-    The canonical MN-major layout (cute/atom/mma_traits_sm100.hpp): in 16-byte units
+    wgmma through an MN-major SWIZZLE_128B descriptor with LBO = one box, SBO = 1024 B and a
+    start-address advance of 2048 B per k16 step (make_desc_sw128, wg::mma_tile).
+    The canonical MN-major layout (cute/atom/mma_traits_sm90_gmma.hpp): in 16-byte units
     ((8,n),(8,k)) : ((1,LBO),(8,SBO)), then Swizzle<3,4,3> on the byte address."""
     BK, CHUNK, ES = 64, 64, 2
     box_bytes = CHUNK * BK * ES            # 8192
     lbo, sbo = box_bytes, 1024
-    mn_extent = 128                        # rows of the operand held by one CTA
+    mn_extent = 128                        # m/n extent of the operand tile of one CTA
     # where TMA puts element (mn, k): box c = mn // 64 starts at c * box_bytes; inside a box row k is
     # 128 bytes long and the whole box is swizzled relative to its 1024-aligned base
     def tma_addr(mn, k):
@@ -139,36 +140,36 @@ def test_mn_major_descriptor_addresses_what_tma_wrote():
 
     # where the MMA with descriptor start address `start` looks for element (mn, k_local) of its
     # 16-deep slice: canonical layout + swizzle of the absolute (1024-aligned) address
-    def umma_addr(start, mn, k_local):
+    def mma_addr(start, mn, k_local):
         e, a, nn = mn % 8, (mn // 8) % 8, mn // 64
         off = e * ES + a * 16 + nn * lbo + (k_local % 8) * 128 + (k_local // 8) * sbo
         return _swizzle128(start + off)
 
     for kstep in range(BK // 16):
-        start = kstep * 2048               # koff in the issue loop: (k * UMMA_K * 128) >> 4 descriptor units
+        start = kstep * 2048               # start-address advance of the issue loop: two 8-row swizzle atoms
         for mn in range(mn_extent):
             for k_local in range(16):
-                assert umma_addr(start, mn, k_local) == tma_addr(mn, kstep * 16 + k_local), (kstep, mn, k_local)
+                assert mma_addr(start, mn, k_local) == tma_addr(mn, kstep * 16 + k_local), (kstep, mn, k_local)
 
 
 def test_k_major_descriptor_addresses_what_tma_wrote():
-    """Same check for the validated K-major GEMM (make_smem_desc_k_sw128): TMA box {64 k, rows},
-    descriptor SBO = 1024 B (8 rows), start-address advance of 32 B per UMMA_K = 16 inside the
+    """Same check for the K-major operands (make_desc_sw128): TMA box {64 k, rows},
+    descriptor SBO = 1024 B (8 rows), start-address advance of 32 B per k16 step inside the
     128-byte swizzle span.  Canonical K-major layout: ((8,m),(T,2)) : ((8T,SBO),(1,T)) elements."""
     ES, rows = 2, 128
 
     def tma_addr(r, k):
         return _swizzle128(r * 128 + k * ES)
 
-    def umma_addr(start, r, k_local):
+    def mma_addr(start, r, k_local):
         off = (r % 8) * 128 + (r // 8) * 1024 + k_local * ES
-        return _swizzle128(start + off)  # the hardware swizzles the final address (validated on B200 for this kernel)
+        return _swizzle128(start + off)  # the hardware swizzles the final address
 
     for kstep in range(4):
         start = kstep * 32
         for r in range(rows):
             for k_local in range(16):
-                assert umma_addr(start, r, k_local) == tma_addr(r, kstep * 16 + k_local)
+                assert mma_addr(start, r, k_local) == tma_addr(r, kstep * 16 + k_local)
 
 
 @pytest.mark.parametrize("nslots,send_blocks,recv_blocks,messages", [(4, 3, 2, [5, 1, 9]), (16, 32, 32, [64, 3]), (2, 1, 5, [7])])
@@ -307,39 +308,25 @@ def test_p2p_copy_engine_groups_and_flags(nslots, messages):
 
 
 def test_push_epilogue_box_coordinates_cover_the_staging_area_once():
-    """Peer-store mode of the fused backward (2-3 ranks): every epilogue warp of every work unit TMA-stores four
-    {64 columns x 32 rows} boxes into the owner's staging area for this source rank, laid out as [ksplit * N rows,
-    K columns].  Mirror of the coordinates in wgrad_bf16_nt_2cta_kernel: each element of part h of tile t is written
-    exactly once and only for the parts the schedule produces."""
-    N, K, ksplit, num_clusters = 1024, 512, 2, 3
-    n_tiles, k_tiles = N // BM2, K // BN
+    """Peer-store mode of the fused backward (2-3 ranks): every consumer warp of every work unit stores its
+    {16 rows x 128 columns} accumulator fragment into the owner's staging area for this source rank, laid out as
+    [ksplit * N rows, K columns].  Mirror of the coordinates in wgrad_bf16_wgmma_kernel: each element of part h
+    of tile t is written exactly once and only for the parts the schedule produces."""
+    N, K, ksplit, num_ctas = 1024, 512, 2, 3
+    n_tiles, k_tiles = N // BM, K // BN
     num_tiles = n_tiles * k_tiles
-    sched = make_sched(num_tiles, num_clusters, ksplit)
+    sched = make_sched(num_tiles, num_ctas, ksplit)
     area = np.zeros((ksplit * N, K), dtype=np.int8)
     for u in range(sched[2]):
         t, h, parts = unit_to_tile(sched, u)
         n_blk, k_blk = divmod(t, k_tiles)
-        for cta, q in itertools.product(range(2), range(4)):
-            row0 = h * N + n_blk * BM2 + cta * BMC + q * 32
-            for c2 in range(BN // 64):
-                col0 = k_blk * BN + c2 * 64
-                area[row0:row0 + 32, col0:col0 + 64] += 1
+        for wgi, w in itertools.product(range(2), range(4)):
+            row0 = h * N + n_blk * BM + wgi * 64 + w * WARP_ROWS
+            col0 = k_blk * BN
+            area[row0:row0 + WARP_ROWS, col0:col0 + BN] += 1
     for t in range(num_tiles):
         n_blk, k_blk = divmod(t, k_tiles)
         parts = 1 if t < sched[0] else sched[1]
         for h in range(ksplit):
-            blk = area[h * N + n_blk * BM2:h * N + (n_blk + 1) * BM2, k_blk * BN:(k_blk + 1) * BN]
+            blk = area[h * N + n_blk * BM:h * N + (n_blk + 1) * BM, k_blk * BN:(k_blk + 1) * BN]
             assert (blk == (1 if h < parts else 0)).all(), (t, h)
-
-
-def test_swizzled_epilogue_box_is_bank_conflict_free_and_matches_tma_swizzle():
-    """The epilogue writes row r's 16-byte chunk j of a {32 rows x 128 bytes} box at r*128 + ((j ^ (r & 7)) << 4):
-    that is exactly TMA's SWIZZLE_128B (Swizzle<3,4,3> of the byte offset), and for a fixed j the 32 lanes of a warp
-    spread over all 8 sixteen-byte bank groups (4 lanes each = the minimum of 4 wavefronts for 512 bytes)."""
-    for j in range(8):
-        groups = {}
-        for r in range(32):
-            addr = r * 128 + ((j ^ (r & 7)) << 4)
-            assert addr == _swizzle128(r * 128 + j * 16)
-            groups.setdefault((addr % 128) // 16, []).append(r)
-        assert len(groups) == 8 and all(len(v) == 4 for v in groups.values())
