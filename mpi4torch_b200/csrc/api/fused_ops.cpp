@@ -43,21 +43,6 @@ Tensor gemm_bf16_tn(const Tensor& x, const Tensor& w) {
   return y;
 }
 
-// Same GEMM on CTA pairs (clusters of two sharing the B tile by TMA multicast); exposed separately for A/B testing.
-Tensor gemm_bf16_tn_2cta(const Tensor& x, const Tensor& w) {
-  check_2d_bf16(x, "x");
-  check_2d_bf16(w, "w");
-  TORCH_CHECK(x.size(1) == w.size(1), "mpi4torch_b200: inner dimensions differ");
-  c10::cuda::CUDAGuard guard(x.device());
-  Tensor y = at::empty({x.size(0), w.size(0)}, x.options());
-  if (y.numel() == 0) return y;
-  std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
-  launch_gemm_bf16_tn_2cta(x.data_ptr(), w.data_ptr(), y.data_ptr(), x.size(0), w.size(0), x.size(1), x.stride(0),
-                           w.stride(0), y.stride(0), backend().device_comm().sm_count,
-                           c10::cuda::getCurrentCUDAStream(x.device().index()).stream());
-  return y;
-}
-
 // y = a @ b with both operands row-major (dgrad: gy[M,N] @ W[N,K]); the weight is read in place through an
 // MN-major wgmma operand, no transposed copy.
 bool gemm_bf16_nn_ok(const Tensor& a, const Tensor& b) {
@@ -312,7 +297,6 @@ TORCH_LIBRARY_FRAGMENT(mpi4torch_b200, m) {
   m.def("gemm_bf16_tn(Tensor x, Tensor w) -> Tensor", &gemm_bf16_tn);
   m.def("gemm_bf16_nn(Tensor a, Tensor b) -> Tensor", &gemm_bf16_nn);
   m.def("gemm_bf16_nn_supported(Tensor a, Tensor b) -> bool", &gemm_bf16_nn_ok);
-  m.def("gemm_bf16_tn_2cta(Tensor x, Tensor w) -> Tensor", &gemm_bf16_tn_2cta);
   m.def("gemm_bf16_tn_supported(Tensor x, Tensor w) -> bool", &gemm_bf16_tn_ok);
   m.def("allreduce_linear_supported(Tensor x, Tensor w) -> bool", &allreduce_linear_supported);
   m.def("allreduce_linear_fused(Tensor x, Tensor w, float scale) -> (Tensor, Tensor)", &allreduce_linear_fused);

@@ -5,12 +5,11 @@
 // (fused_allreduce_gemm, below).
 //
 // Structure: see wgmma_pipeline.cuh (persistent CTAs, 128x256 tiles - 128x128 in the fused
-// kernel -, TMA producer warp, two consumer warpgroups; CL = 2: CTA pairs in a cluster on
-// 256x256 tiles, B multicast).  Fused kernel only: four communication warps run the NVLS
-// reduce of weight panels (multimem.ld_reduce over all ranks' weights -> x 1/size ->
-// multimem.st into every rank's W_avg -> multimem.red on the panel counter).  The TMA
-// producer polls that counter before loading from a panel, so the all-reduce of panel
-// p+1.. overlaps the MMAs on panel p.
+// kernel -, TMA producer warp, two consumer warpgroups).  Fused kernel only: four
+// communication warps run the NVLS reduce of weight panels (multimem.ld_reduce over all
+// ranks' weights -> x 1/size -> multimem.st into every rank's W_avg -> multimem.red on the
+// panel counter).  The TMA producer polls that counter before loading from a panel, so the
+// all-reduce of panel p+1.. overlaps the MMAs on panel p.
 #include <cuda.h>
 
 #include <algorithm>
@@ -48,23 +47,20 @@ struct GemmArgs {
 // the fused kernel's communication warps need registers: half-width tiles there
 template <bool FUSED> constexpr int tile_n() { return FUSED ? 128 : 256; }
 
-// CL = 2: launched as clusters of two CTAs (launch_pair below); each pair works on 256-row tiles.
-template <bool FUSED, int EPI, bool B_MN, int CL = 1>
+template <bool FUSED, int EPI, bool B_MN>
 __global__ void __launch_bounds__(kGemmThreads + (FUSED ? kCommWarps * 32 : 0), 1)
 gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                        const GemmArgs g, const CommArgs cm) {
-  static_assert(CL == 1 || !FUSED, "the fused kernel runs on single CTAs");
   constexpr int BN = tile_n<FUSED>();
-  constexpr int TM = BM * CL;  // rows of a tile
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = aligned_smem(smem_raw);
   Pipe* pipe = pipe_of<BN>(smem);
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t crank = CL == 2 ? tc::cluster_ctarank() : 0u;
-  const int group = blockIdx.x / CL, num_groups = gridDim.x / CL;  // both CTAs of a pair walk the same tiles
+  // read once for both roles: reading them inside each branch costs the fused kernel ten registers
+  const int first_tile = blockIdx.x, tile_stride = gridDim.x;
 
-  const int m_tiles = (g.M + TM - 1) / TM;
+  const int m_tiles = (g.M + BM - 1) / BM;
   const int n_tiles = (g.N + BN - 1) / BN;
   const int num_tiles = m_tiles * n_tiles;
   const int k_blocks = (g.K + BK - 1) / BK;
@@ -72,40 +68,25 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
   if (warp == 0 && lane == 0) {
     tc::prefetch_tmap(&tmap_a);
     tc::prefetch_tmap(&tmap_b);
-    init_pipe<BN, CL>(pipe);
+    init_pipe<BN>(pipe);
   }
-  if (CL == 2) tc::cluster_sync();  // the peer's barriers exist before anything is multicast into them
-  else __syncthreads();
+  __syncthreads();
 
   if (warp < 4) {
     // =========================== TMA producer ===========================
     if (warp == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int t = group; t < num_tiles; t += num_groups) {
+      for (int t = first_tile; t < num_tiles; t += tile_stride) {
         const int n_blk = t / m_tiles;  // M fastest: a wave works on few weight panels
         const int m_blk = t - n_blk * m_tiles;
         if (FUSED) {
           // the weight panel must have been all-reduced (by every rank) first
-          const uint32_t* flag = g.panel_flags + n_blk * BN / kPanel;
-          // bounded like every other cross-rank wait: a peer that never publishes
-          // must end in an error, not in a hung GPU
-          if (static_cast<int32_t>(ld_acquire_sys_u32(flag) - g.panel_target) < 0) {
-            const unsigned long long t0 = globaltimer_ns();
-            unsigned int spins = 0;
-            while (static_cast<int32_t>(ld_acquire_sys_u32(flag) - g.panel_target) < 0) {
-              if ((++spins & 0x3ff) == 0 && globaltimer_ns() - t0 > cm.sync.timeout_ns) {
-                *reinterpret_cast<volatile int*>(cm.sync.err_flag) = kErrTimeout;
-                __threadfence_system();
-                __trap();
-              }
-            }
-          }
+          bounded_wait_ge(g.panel_flags + n_blk * BN / kPanel, g.panel_target, cm.sync);
           tc::fence_proxy_async();  // generic-proxy writes (multimem.st) -> async-proxy reads (TMA)
         }
         for (int kb = 0; kb < k_blocks; ++kb)
-          load_stage<false, B_MN, BN, CL>(smem, pipe, stage, phase, &tmap_a, &tmap_b, m_blk * TM + crank * BM, n_blk * BN,
-                                          kb * BK, crank);
+          load_stage<false, B_MN, BN>(smem, pipe, stage, phase, &tmap_a, &tmap_b, m_blk * BM, n_blk * BN, kb * BK);
       }
     }
   } else if (warp < kGemmThreads / 32) {
@@ -114,14 +95,14 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     int stage = 0;
     uint32_t phase = 0;
     float acc[BN / 2];
-    for (int t = group; t < num_tiles; t += num_groups) {
+    for (int t = first_tile; t < num_tiles; t += tile_stride) {
       const int n_blk = t / m_tiles;
       const int m_blk = t - n_blk * m_tiles;
-      mma_tile<false, B_MN, BN, CL>(acc, smem, pipe, stage, phase, k_blocks, wgi, crank);
+      mma_tile<false, B_MN, BN>(acc, smem, pipe, stage, phase, k_blocks, wgi);
       float loss_part = 0.f;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const int row = m_blk * TM + static_cast<int>(crank) * BM + wgi * 64 + frag_row(h);
+        const int row = m_blk * BM + wgi * 64 + frag_row(h);
         if (row >= g.M) continue;
         uint16_t* crow = static_cast<uint16_t*>(g.C) + static_cast<int64_t>(row) * g.ldc;
         const uint16_t* trow = EPI == 1 ? static_cast<const uint16_t*>(g.T) + static_cast<int64_t>(row) * g.ldt : nullptr;
@@ -163,8 +144,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     // =========================== communication ==========================
     comm_allreduce_panels<kCommWarps, kPanel>(cm, kGemmThreads, g.N / kPanel, g.K);
   }
-  if (CL == 2) tc::cluster_sync();  // the peer may still multicast into / arrive on this CTA's barriers
-  else __syncthreads();
+  __syncthreads();
 }
 
 // ---------------------------------------------------------------------------
@@ -177,10 +157,10 @@ CUtensorMap make_tmap(const void* base, int64_t rows, int64_t cols, int64_t ld, 
 
 template <bool FUSED> constexpr int smem_bytes() { return Tile<tile_n<FUSED>()>::kSmemBytes; }
 
-template <bool FUSED, int EPI, bool B_MN, int CL = 1> void configure_once() {
+template <bool FUSED, int EPI, bool B_MN> void configure_once() {
   static std::once_flag once;
   std::call_once(once, [] {
-    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<FUSED, EPI, B_MN, CL>,
+    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<FUSED, EPI, B_MN>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes<FUSED>());
     M4T_CHECK(e == cudaSuccess, "cudaFuncSetAttribute(smem) failed: " << cudaGetErrorString(e));
   });
@@ -193,30 +173,6 @@ void launch(int grid, const CUtensorMap& ta, const CUtensorMap& tb, const GemmAr
   gemm_bf16_wgmma_kernel<FUSED, EPI, B_MN>
       <<<grid, kGemmThreads + (FUSED ? kCommWarps * 32 : 0), smem_bytes<FUSED>(), stream>>>(ta, tb, g, cm);
   cudaError_t e = cudaGetLastError();
-  M4T_CHECK(e == cudaSuccess, what << " launch failed: " << cudaGetErrorString(e));
-  note_kernel_launch(what);
-}
-
-// Clusters of two CTAs (`pairs` of them) for the CL = 2 kernel.
-template <int EPI>
-void launch_pair(int pairs, const CUtensorMap& ta, const CUtensorMap& tb, const GemmArgs& g, cudaStream_t stream,
-                 const char* what) {
-  configure_once<false, EPI, false, 2>();
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(2 * pairs, 1, 1);
-  cfg.blockDim = dim3(kGemmThreads, 1, 1);
-  cfg.dynamicSmemBytes = smem_bytes<false>();
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, gemm_bf16_wgmma_kernel<false, EPI, false, 2>, ta, tb, g, CommArgs{});
-  M4T_CHECK(e == cudaSuccess, what << " launch failed: " << cudaGetErrorString(e));
-  e = cudaGetLastError();
   M4T_CHECK(e == cudaSuccess, what << " launch failed: " << cudaGetErrorString(e));
   note_kernel_launch(what);
 }
@@ -257,29 +213,6 @@ void launch_gemm_bf16_tn(const void* A, const void* B, void* C, int64_t M, int64
     launch<false, 1, false>(grid, ta, tb, g, CommArgs{}, stream, "gemm_mse_epilogue");
   } else {
     launch<false, 0, false>(grid, ta, tb, g, CommArgs{}, stream, "gemm_bf16_tn");
-  }
-}
-
-// Same contract on CTA pairs: 256x256 tiles, each CTA loads half of the B tile and multicasts it to both.
-void launch_gemm_bf16_tn_2cta(const void* A, const void* B, void* C, int64_t M, int64_t N, int64_t K, int64_t lda,
-                              int64_t ldb, int64_t ldc, int sm_count, cudaStream_t stream, const MseEpilogue* mse) {
-  M4T_CHECK(gemm_bf16_tn_supported(M, N, K, A, B, C, lda, ldb, ldc), "unsupported GEMM shape/alignment for the wgmma path");
-  constexpr int BN = tile_n<false>();
-  const CUtensorMap ta = make_tmap(A, M, K, lda, BM);
-  const CUtensorMap tb = make_tmap(B, N, K, ldb, BN / 2);  // each CTA of the pair loads half of the B tile
-  GemmArgs g{};
-  g.C = C;
-  g.M = static_cast<int>(M);
-  g.N = static_cast<int>(N);
-  g.K = static_cast<int>(K);
-  g.ldc = static_cast<int>(ldc);
-  const int tiles = static_cast<int>(((M + 2 * BM - 1) / (2 * BM)) * ((N + BN - 1) / BN));
-  const int pairs = std::max(1, std::min(tiles, sm_count / 2));
-  if (mse) {
-    set_mse(g, mse);
-    launch_pair<1>(pairs, ta, tb, g, stream, "gemm_2cta_mse_epilogue");
-  } else {
-    launch_pair<0>(pairs, ta, tb, g, stream, "gemm_2cta");
   }
 }
 

@@ -59,36 +59,6 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
-// Same load, written at the same shared-memory offset into every CTA of the cluster named in `cta_mask`;
-// each destination CTA's mbarrier at `bar`'s offset receives the transaction bytes of its copy.
-__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int32_t c0,
-                                                      int32_t c1, uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1),
-        "h"(cta_mask)
-      : "memory");
-}
-
-// ---- thread-block clusters ----------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-// Every thread of every CTA of the cluster; orders the barrier initialisation / the last remote accesses.
-__device__ __forceinline__ void cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// Arrive on the mbarrier at `bar`'s offset inside CTA `rank` of the cluster.
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t rank) {
-  uint32_t remote;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(rank));
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
-}
-
 // ---- wgmma descriptors -------------------------------------------------------------
 // Operand tiles are written by TMA with SWIZZLE_128B: 128-byte rows, 8-row (1024 B) swizzle atoms.
 // GMMA descriptor: start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), base offset [49,52) (0: atoms are

@@ -118,9 +118,6 @@ struct MseEpilogue {
 // C[M,N] = A[M,K] * B[N,K]^T, bf16 in / fp32 accumulate / bf16 out.
 void launch_gemm_bf16_tn(const void* A, const void* B, void* C, int64_t M, int64_t N, int64_t K, int64_t lda,
                          int64_t ldb, int64_t ldc, int sm_count, cudaStream_t stream, const MseEpilogue* mse = nullptr);
-// Same contract on CTA pairs (clusters of two, 256x256 tiles, B tile multicast to both CTAs).
-void launch_gemm_bf16_tn_2cta(const void* A, const void* B, void* C, int64_t M, int64_t N, int64_t K, int64_t lda,
-                              int64_t ldb, int64_t ldc, int sm_count, cudaStream_t stream, const MseEpilogue* mse = nullptr);
 // y = x @ (scale * sum_ranks W)^T in one kernel; W staged at heap offset w_off on every rank.
 void launch_fused_allreduce_gemm(const DeviceComm& dc, const void* x, void* y, int64_t M, int64_t N, int64_t K,
                                  int64_t ldx, int64_t ldy, int64_t w_off, int64_t wavg_off, int64_t flags_off,

@@ -6,10 +6,6 @@
 //   warpgroups 1, 2                 consumers: 64 rows each, wgmma m64nBNk16 into BN/2 fp32
 //                                   registers per thread, epilogue straight from registers
 //   further warps                   (fused kernels only) communication role
-// CL = 2 runs the same loop on a cluster of two CTAs that share one 256 x BN tile: each CTA
-// stages its own 128 rows of A and loads HALF of the B tile, multicast by TMA into both CTAs,
-// so a pair moves 2/3 of the L2 -> SMEM bytes of two independent CTAs.  A stage may only be
-// refilled when the consumers of BOTH CTAs released it: the empty barriers count both.
 // Each operand is either K-major (one TMA box {64 k, rows}) or MN-major (boxes of
 // {64 contiguous m/n, 64 k-rows}); the wgmma transpose bits select the layout, so no
 // operand is ever copied transposed.
@@ -47,10 +43,10 @@ template <int BN> __device__ __forceinline__ Pipe* pipe_of(uint8_t* smem) {
   return reinterpret_cast<Pipe*>(smem + Tile<BN>::kStages * Tile<BN>::kStageBytes);
 }
 
-template <int BN, int CL = 1> __device__ __forceinline__ void init_pipe(Pipe* p) {
+template <int BN> __device__ __forceinline__ void init_pipe(Pipe* p) {
   for (int s = 0; s < Tile<BN>::kStages; ++s) {
     tc::mbar_init(&p->full[s], 1);
-    tc::mbar_init(&p->empty[s], kConsumerWarps * CL);  // one arrive per consumer warp of every CTA that writes here
+    tc::mbar_init(&p->empty[s], kConsumerWarps);  // one arrive per consumer warp
   }
   tc::fence_barrier_init();
 }
@@ -63,11 +59,9 @@ template <int BN> __device__ __forceinline__ void advance(int& stage, uint32_t& 
 }
 
 // Producer: one stage = A rows [m0, m0+128) and B rows [n0, n0+BN) of the k-slice starting at k0.
-// CL = 2: this CTA (cluster rank `crank`) loads B rows [n0 + crank*BN/2, +BN/2) into both CTAs.
-template <bool A_MN, bool B_MN, int BN, int CL = 1>
+template <bool A_MN, bool B_MN, int BN>
 __device__ __forceinline__ void load_stage(uint8_t* smem, Pipe* p, int& stage, uint32_t& phase, const CUtensorMap* ma,
-                                           const CUtensorMap* mb, int m0, int n0, int k0, uint32_t crank = 0) {
-  static_assert(CL == 1 || !B_MN, "the CTA pair splits a K-major B tile");
+                                           const CUtensorMap* mb, int m0, int n0, int k0) {
   tc::mbar_wait(&p->empty[stage], phase ^ 1);
   uint8_t* sa = smem + stage * Tile<BN>::kStageBytes;
   uint8_t* sb = sa + kABytes;
@@ -78,10 +72,7 @@ __device__ __forceinline__ void load_stage(uint8_t* smem, Pipe* p, int& stage, u
   } else {
     tc::tma_load_2d(sa, ma, &p->full[stage], k0, m0);
   }
-  if (CL == 2) {
-    const int half = static_cast<int>(crank) * (BN / 2);
-    tc::tma_load_2d_multicast(sb + half * 128, mb, &p->full[stage], k0, n0 + half, 0x3);
-  } else if (B_MN) {
+  if (B_MN) {
 #pragma unroll
     for (int ch = 0; ch < BN / 64; ++ch) tc::tma_load_2d(sb + ch * kBoxBytesMN, mb, &p->full[stage], n0 + ch * 64, k0);
   } else {
@@ -93,16 +84,10 @@ __device__ __forceinline__ void load_stage(uint8_t* smem, Pipe* p, int& stage, u
 // Consumer warpgroup `wgi` (0/1): acc = its 64 rows of the tile, summed over k_blocks stages.
 // The stage of k-block kb is handed back to the producer once the wgmma of kb + 1 has been
 // issued and those of kb have retired (wait_group 1), so one k-block of MMAs is always queued.
-template <bool A_MN, bool B_MN, int BN, int CL = 1>
+template <bool A_MN, bool B_MN, int BN>
 __device__ __forceinline__ void mma_tile(float (&acc)[BN / 2], uint8_t* smem, Pipe* p, int& stage, uint32_t& phase,
-                                         int k_blocks, int wgi, uint32_t crank = 0) {
+                                         int k_blocks, int wgi) {
   const int lane = threadIdx.x & 31;
-  // the stage is free again for every producer that wrote into it: this CTA's and, in a pair, the peer's
-  auto release = [&](int s) {
-    if (lane != 0) return;
-    tc::mbar_arrive(&p->empty[s]);
-    if (CL == 2) tc::mbar_arrive_remote(&p->empty[s], crank ^ 1u);
-  };
   int prev = -1;
   tc::fence_regs(acc);
   for (int kb = 0; kb < k_blocks; ++kb) {
@@ -124,13 +109,13 @@ __device__ __forceinline__ void mma_tile(float (&acc)[BN / 2], uint8_t* smem, Pi
     }
     tc::wgmma_commit();
     tc::wgmma_wait<1>();
-    if (prev >= 0) release(prev);
+    if (prev >= 0 && lane == 0) tc::mbar_arrive(&p->empty[prev]);
     prev = stage;
     advance<BN>(stage, phase);
   }
   tc::wgmma_wait<0>();
   tc::fence_regs(acc);
-  if (prev >= 0) release(prev);
+  if (prev >= 0 && lane == 0) tc::mbar_arrive(&p->empty[prev]);
 }
 
 // Accumulator fragment of wgmma m64nN (fp32): thread (warp w of the warpgroup, lane l) holds, for
@@ -141,6 +126,21 @@ __device__ __forceinline__ int frag_col(int j) { return 8 * j + 2 * (threadIdx.x
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   return static_cast<uint32_t>(float_to_bf16_bits(lo)) | (static_cast<uint32_t>(float_to_bf16_bits(hi)) << 16);
+}
+
+// Cross-rank wait of the fused kernels: spins until *flag >= target (wrap-safe).  A peer that never
+// publishes must end in an error, not in a hung GPU: on timeout the error word is set and the kernel traps.
+__device__ __forceinline__ void bounded_wait_ge(const uint32_t* flag, uint32_t target, const SyncCtx& c) {
+  if (static_cast<int32_t>(ld_acquire_sys_u32(flag) - target) >= 0) return;
+  const unsigned long long t0 = globaltimer_ns();
+  unsigned int spins = 0;
+  while (static_cast<int32_t>(ld_acquire_sys_u32(flag) - target) < 0) {
+    if ((++spins & 0x3ff) == 0 && globaltimer_ns() - t0 > c.timeout_ns) {
+      *reinterpret_cast<volatile int*>(c.err_flag) = kErrTimeout;
+      __threadfence_system();
+      __trap();
+    }
+  }
 }
 
 }  // namespace wg

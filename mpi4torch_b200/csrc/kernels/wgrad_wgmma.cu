@@ -111,19 +111,6 @@ __host__ __device__ inline void unit_to_tile(const UnitSched& s, int u, int& t, 
   }
 }
 
-__device__ __forceinline__ void bounded_wait_ge(const uint32_t* flag, uint32_t target, const SyncCtx& c) {
-  if (static_cast<int32_t>(ld_acquire_sys_u32(flag) - target) >= 0) return;
-  const unsigned long long t0 = globaltimer_ns();
-  unsigned int spins = 0;
-  while (static_cast<int32_t>(ld_acquire_sys_u32(flag) - target) < 0) {
-    if ((++spins & 0x3ff) == 0 && globaltimer_ns() - t0 > c.timeout_ns) {
-      *reinterpret_cast<volatile int*>(c.err_flag) = kErrTimeout;
-      __threadfence_system();
-      __trap();
-    }
-  }
-}
-
 // Owner side of the fused mode; runs on kCommWarps warps of every CTA.
 // MC: reduce through the NVSwitch (multimem.ld_reduce / multimem.st); otherwise NSRC peer loads in rank
 // order and one store per peer (2-3 ranks, or no multicast mapping).
