@@ -1,0 +1,140 @@
+#!/usr/bin/env python
+"""Training step of the data-parallel two-layer MLP (DPMLPModel: Linear -> GELU(tanh) -> Linear, biases, MSE) on
+one GPU, against the eager bf16 composition (two nn.Linear, F.gelu, MSE, loss.backward(), SGD), and each MLP
+epilogue kernel against its plain counterpart on the same shape.  One process; the arms are alternated and timed
+with device events.  Prints one JSON line.
+
+    python benchmarks/mlp_step.py [--batch 8192 --d 4096 --h 16384 --o 4096 --steps 20 --warmup 5 --reps 3]
+"""
+import argparse
+import json
+import os
+import statistics
+import subprocess
+import sys
+
+import torch
+import torch.nn.functional as F
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+import mpi4torch_b200 as m4t  # noqa: E402
+from mpi4torch_b200.models import DPMLPModel  # noqa: E402
+from mpi4torch_b200.utils.timing import ClockSampler  # noqa: E402
+
+
+def time_ms(fn, steps):
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record()
+    for _ in range(steps):
+        fn()
+    b.record()
+    b.synchronize()
+    return a.elapsed_time(b) / steps
+
+
+def card():
+    """Name, power limit and max SM clock, read-only."""
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits",
+                              "-i", str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout
+        name, power, clock = [s.strip() for s in out.strip().splitlines()[0].split(",")]
+        return {"gpu": name, "power_limit_w": float(power), "max_sm_mhz": float(clock)}
+    except (OSError, ValueError, IndexError, subprocess.TimeoutExpired):
+        return {"gpu": torch.cuda.get_device_name(), "power_limit_w": None, "max_sm_mhz": None}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--batch", type=int, default=8192)
+    ap.add_argument("--d", type=int, default=4096)
+    ap.add_argument("--h", type=int, default=16384)
+    ap.add_argument("--o", type=int, default=4096)
+    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--reps", type=int, default=3, help="alternations of the arms; medians are reported")
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("mlp_step.py needs a GPU")
+    comm = m4t.COMM_WORLD
+    if not m4t.cuda_backend_ready():
+        raise SystemExit("the native CUDA backend did not initialise")
+    B, D, H, O = args.batch, args.d, args.h, args.o
+    ops = torch.ops.mpi4torch_b200
+    g = torch.Generator(device="cuda").manual_seed(0)
+    x = torch.randn(B, D, device="cuda", generator=g).to(torch.bfloat16)
+    t = torch.randn(B, O, device="cuda", generator=g).to(torch.bfloat16)
+    lr = 1e-4
+
+    model = DPMLPModel(D, H, O, comm, device="cuda", lr=lr, seed=0)
+    if not model._in_backward(x, t):
+        raise SystemExit(f"shape {(B, D, H, O)} is off the MLP kernel path")
+
+    lin1 = torch.nn.Linear(D, H, device="cuda", dtype=torch.bfloat16)
+    lin2 = torch.nn.Linear(H, O, device="cuda", dtype=torch.bfloat16)
+    eager_params = list(lin1.parameters()) + list(lin2.parameters())
+
+    def eager_step():
+        y = lin2(F.gelu(lin1(x), approximate="tanh"))
+        loss = (y.float() - t.float()).square().mean()
+        loss.backward()
+        with torch.no_grad():
+            grads = [p.grad for p in eager_params]
+            torch._foreach_add_(eager_params, grads, alpha=-lr)
+        for p in eager_params:
+            p.grad = None
+
+    # each MLP kernel and its plain counterpart on the same shape
+    w1, b1 = model.w1.detach(), model.b1.detach()
+    w2, b2 = model.w2.detach(), model.b2.detach()
+    h, z = ops.linear_bias_gelu_forward(x, w1, b1)
+    dy, _, _ = ops.linear_bias_mse_forward_local(h, w2, b2, t, 1.0 / B, 2.0 / B)
+    pairs = {
+        "gemm_bias_gelu": (lambda: ops.linear_bias_gelu_forward(x, w1, b1), lambda: ops.gemm_bf16_tn(x, w1)),
+        "gemm_bias_mse_colsum": (lambda: ops.linear_bias_mse_forward_local(h, w2, b2, t, 1.0 / B, 2.0 / B),
+                                 lambda: ops.linear_mse_forward_local(h, w2, t, 1.0 / B, 2.0 / B)),
+        "gemm_nn_gelu_bwd_colsum": (lambda: ops.gemm_nn_gelu_backward(dy, w2, z), lambda: ops.gemm_bf16_nn(dy, w2)),
+    }
+
+    arms = {"model": lambda: model.train_step(x, t), "eager": eager_step}
+    for name, (new, plain) in pairs.items():
+        arms[name] = new
+        arms[name + ":plain"] = plain
+    for fn in arms.values():  # warm every shape: module loading, allocator, cuBLAS heuristics
+        for _ in range(args.warmup):
+            fn()
+    torch.cuda.synchronize()
+
+    table0 = dict(m4t._C.kernel_launch_table())
+    time_ms(arms["model"], 1)
+    kernels_per_step = {k: v - table0.get(k, 0) for k, v in dict(m4t._C.kernel_launch_table()).items()
+                        if v - table0.get(k, 0) > 0}
+
+    sampler = ClockSampler(gpu_index=torch.cuda.current_device()).start()
+    samples = {k: [] for k in arms}
+    for _ in range(args.reps):
+        for name, fn in arms.items():
+            samples[name].append(time_ms(fn, args.steps))
+    clocks = sampler.stop()
+    ms = {k: statistics.median(v) for k, v in samples.items()}
+
+    gemm_flop = 2.0 * B * (2 * H * D + 3 * H * O)  # fwd1 + wgrad1 over H*D, fwd2 + dgrad2 + wgrad2 over H*O
+    res = {
+        "shape": {"B": B, "D": D, "H": H, "O": O},
+        "model_ms_per_step": round(ms["model"], 4),
+        "model_tflops": round(gemm_flop / ms["model"] / 1e9, 1),
+        "eager_ms_per_step": round(ms["eager"], 4),
+        "eager_tflops": round(gemm_flop / ms["eager"] / 1e9, 1),
+        "kernels": {name: {"ms": round(ms[name], 4), "plain_ms": round(ms[name + ":plain"], 4),
+                           "overhead": round(ms[name] / ms[name + ":plain"] - 1.0, 4)} for name in pairs},
+        "kernels_per_step": kernels_per_step,
+        "spread_ms": {k: [round(min(v), 4), round(max(v), 4)] for k, v in samples.items()},
+        "sm_mhz_median": clocks.get("sm_mhz"),
+        "throttle_reasons": clocks.get("reasons"),
+        **card(),
+    }
+    print(json.dumps(res), flush=True)
+
+
+if __name__ == "__main__":
+    main()

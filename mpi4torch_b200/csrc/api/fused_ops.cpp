@@ -276,9 +276,109 @@ std::tuple<Tensor, Tensor> linear_mse_forward_local(const Tensor& x, const Tenso
   return {dy, loss};
 }
 
+// ---- two-layer MLP (Linear -> GELU(tanh) -> Linear, MSE) ------------------------------------------
+void check_bias(const Tensor& b, const Tensor& w) {
+  TORCH_CHECK(b.is_cuda() && b.device() == w.device() && b.dim() == 1 && b.scalar_type() == at::kFloat &&
+                  b.is_contiguous() && b.size(0) == w.size(0),
+              "mpi4torch_b200: the bias must be a contiguous fp32 CUDA vector of the weight's output size");
+}
+
+Tensor colsum_workspace(int64_t M, int64_t N, const Tensor& like) {
+  return at::empty({colsum_rows(M), N}, like.options().dtype(at::kFloat));
+}
+
+// (h, z) with z = x @ w^T + b and h = gelu_tanh(z), both bf16; h is computed from the fp32 z.
+std::tuple<Tensor, Tensor> linear_bias_gelu_forward(const Tensor& x, const Tensor& w, const Tensor& b) {
+  check_2d_bf16(x, "x");
+  check_2d_bf16(w, "w");
+  check_bias(b, w);
+  TORCH_CHECK(x.size(1) == w.size(1), "mpi4torch_b200: inner dimensions differ");
+  c10::cuda::CUDAGuard guard(x.device());
+  Tensor z = at::empty({x.size(0), w.size(0)}, x.options());
+  Tensor h = at::empty_like(z);
+  if (z.numel() == 0) return {h, z};
+  std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
+  launch_gemm_bias_gelu(x.data_ptr(), w.data_ptr(), b.data_ptr<float>(), z.data_ptr(), h.data_ptr(), x.size(0), w.size(0),
+                        x.size(1), x.stride(0), w.stride(0), z.stride(0), backend().device_comm().sm_count,
+                        c10::cuda::getCurrentCUDAStream(x.device().index()).stream());
+  return {h, z};
+}
+
+// Forward of the output layer with the MSE epilogue, against already averaged parameters:
+//   dy = grad_scale * (x @ w^T + b - target)  (bf16),  loss[1] = loss_scale * sum((x @ w^T + b - target)^2),
+//   partials = fp32 column-sum partials of dy (reduce them with column_sum).
+std::tuple<Tensor, Tensor, Tensor> linear_bias_mse_forward_local(const Tensor& x, const Tensor& w, const Tensor& b,
+                                                                 const Tensor& target, double loss_scale,
+                                                                 double grad_scale) {
+  check_2d_bf16(x, "x");
+  check_2d_bf16(w, "w");
+  check_2d_bf16(target, "target");
+  check_bias(b, w);
+  TORCH_CHECK(x.size(1) == w.size(1) && target.size(0) == x.size(0) && target.size(1) == w.size(0),
+              "mpi4torch_b200: linear_bias_mse_forward_local shape mismatch");
+  TORCH_CHECK(x.size(0) > 0, "mpi4torch_b200: linear_bias_mse_forward_local needs a non-empty batch");
+  c10::cuda::CUDAGuard guard(x.device());
+  Tensor dy = at::empty({x.size(0), w.size(0)}, x.options());
+  Tensor loss = at::zeros({1}, x.options().dtype(at::kFloat));
+  Tensor part = colsum_workspace(x.size(0), w.size(0), x);
+  MseEpilogue mse;
+  mse.target = target.data_ptr();
+  mse.ldt = target.stride(0);
+  mse.loss_acc = loss.data_ptr<float>();
+  mse.loss_scale = static_cast<float>(loss_scale);
+  mse.grad_scale = static_cast<float>(grad_scale);
+  std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
+  launch_gemm_bias_mse_colsum(x.data_ptr(), w.data_ptr(), b.data_ptr<float>(), dy.data_ptr(), part.data_ptr<float>(),
+                              x.size(0), w.size(0), x.size(1), x.stride(0), w.stride(0), dy.stride(0),
+                              backend().device_comm().sm_count, c10::cuda::getCurrentCUDAStream(x.device().index()).stream(),
+                              mse);
+  return {dy, loss, part};
+}
+
+// (dz, partials): dz = grad_scale * (dy @ w) * gelu_tanh'(z) in bf16 (w read in place as in gemm_bf16_nn), and the
+// fp32 column-sum partials of dz.
+std::tuple<Tensor, Tensor> gemm_nn_gelu_backward(const Tensor& dy, const Tensor& w, const Tensor& z,
+                                                 const c10::optional<Tensor>& grad_scale) {
+  check_2d_bf16(dy, "dy");
+  check_2d_bf16(w, "w");
+  check_2d_bf16(z, "z");
+  TORCH_CHECK(dy.size(1) == w.size(0) && z.size(0) == dy.size(0) && z.size(1) == w.size(1),
+              "mpi4torch_b200: gemm_nn_gelu_backward shape mismatch");
+  TORCH_CHECK(dy.size(0) > 0, "mpi4torch_b200: gemm_nn_gelu_backward needs a non-empty batch");
+  c10::cuda::CUDAGuard guard(dy.device());
+  Tensor dz = at::empty({dy.size(0), w.size(1)}, dy.options());
+  Tensor part = colsum_workspace(dy.size(0), w.size(1), dy);
+  std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
+  launch_gemm_nn_gelu_bwd_colsum(dy.data_ptr(), w.data_ptr(), z.data_ptr(), dz.data_ptr(), part.data_ptr<float>(), dy.size(0),
+                                 w.size(1), dy.size(1), dy.stride(0), w.stride(0), z.stride(0), dz.stride(0),
+                                 backend().device_comm().sm_count,
+                                 c10::cuda::getCurrentCUDAStream(dy.device().index()).stream(), grad_scale_ptr(grad_scale, dy));
+  return {dz, part};
+}
+
+// out[n] = grad_scale * sum_i partials[i, n] (fp32), in a fixed order of i: bit-identical on every call.
+Tensor column_sum(const Tensor& partials, const c10::optional<Tensor>& grad_scale) {
+  TORCH_CHECK(partials.is_cuda() && partials.dim() == 2 && partials.scalar_type() == at::kFloat && partials.is_contiguous() &&
+                  partials.size(0) > 0,
+              "mpi4torch_b200: column_sum needs a non-empty contiguous 2-d fp32 CUDA tensor");
+  c10::cuda::CUDAGuard guard(partials.device());
+  Tensor out = at::empty({partials.size(1)}, partials.options());
+  if (out.numel() == 0) return out;
+  launch_column_sum(partials.data_ptr<float>(), partials.size(0), partials.size(1), out.data_ptr<float>(),
+                    grad_scale_ptr(grad_scale, partials), c10::cuda::getCurrentCUDAStream(partials.device().index()).stream());
+  return out;
+}
+
 }  // namespace
 
 TORCH_LIBRARY_FRAGMENT(mpi4torch_b200, m) {
+  m.def("linear_bias_gelu_forward(Tensor x, Tensor w, Tensor b) -> (Tensor, Tensor)", &linear_bias_gelu_forward);
+  m.def("linear_bias_mse_forward_local(Tensor x, Tensor w, Tensor b, Tensor target, float loss_scale, float grad_scale) "
+        "-> (Tensor, Tensor, Tensor)",
+        &linear_bias_mse_forward_local);
+  m.def("gemm_nn_gelu_backward(Tensor dy, Tensor w, Tensor z, Tensor? grad_scale=None) -> (Tensor, Tensor)",
+        &gemm_nn_gelu_backward);
+  m.def("column_sum(Tensor partials, Tensor? grad_scale=None) -> Tensor", &column_sum);
   m.def("wgrad_allreduce_sgd_prefetch_(Tensor(a!) w, Tensor dy, Tensor x, float scale, Tensor? grad_scale=None) -> Tensor",
         &wgrad_allreduce_sgd_prefetch_);
   m.def("wgrad_sgd_(Tensor(a!) w, Tensor dy, Tensor x, float scale, Tensor? grad_scale=None) -> ()", &wgrad_sgd_);

@@ -124,6 +124,26 @@ void launch_fused_allreduce_gemm(const DeviceComm& dc, const void* x, void* y, i
                                  uint32_t panel_target, float scale, cudaStream_t stream, const MseEpilogue* mse = nullptr);
 int fused_gemm_grid(const DeviceComm& dc);
 
+// ---- epilogues of the two-layer MLP (gemm_wgmma.cu) -----------------------------------
+// Column sums come as fp32 partials [colsum_rows(M), N] (one row per 16 output rows, deterministic);
+// launch_column_sum reduces them in a fixed order.
+int64_t colsum_rows(int64_t M);
+// z = A[M,K] * B[N,K]^T + bias, h = gelu_tanh(z) (from the fp32 z); z and h bf16 with leading dimension ldc.
+void launch_gemm_bias_gelu(const void* A, const void* B, const float* bias, void* z, void* h, int64_t M, int64_t N,
+                           int64_t K, int64_t lda, int64_t ldb, int64_t ldc, int sm_count, cudaStream_t stream);
+// dy = grad_scale * (A * B^T + bias - target), loss as MseEpilogue, colsum = partial column sums of dy.
+void launch_gemm_bias_mse_colsum(const void* A, const void* B, const float* bias, void* dy, float* colsum, int64_t M,
+                                 int64_t N, int64_t K, int64_t lda, int64_t ldb, int64_t ldc, int sm_count,
+                                 cudaStream_t stream, const MseEpilogue& mse);
+// dz = gscale * (A[M,K] * B[K,N]) * gelu_tanh'(z)  (B row-major, read MN-major; z bf16 [M,N]),
+// colsum = partial column sums of dz.
+void launch_gemm_nn_gelu_bwd_colsum(const void* A, const void* B, const void* z, void* dz, float* colsum, int64_t M,
+                                    int64_t N, int64_t K, int64_t lda, int64_t ldb, int64_t ldz, int64_t ldc,
+                                    int sm_count, cudaStream_t stream, const float* gscale = nullptr);
+// out[n] = gscale * sum_i partial[i, n], fp32, summed in a fixed order of i.
+void launch_column_sum(const float* partial, int64_t rows, int64_t N, float* out, const float* gscale,
+                       cudaStream_t stream);
+
 // ---- weight gradient (wgrad_wgmma.cu) ------------------------------------------------
 // G[N,K] = dY[Mb,N]^T * X[Mb,K]: both operands MN-major, no transposed copies.
 bool wgrad_bf16_supported(int64_t Mb, int64_t N, int64_t K, const void* dy, const void* x, const void* g, int64_t ldy,

@@ -405,9 +405,14 @@ bool CudaBackend::fused_wgrad_available(const void* w, int64_t Mb, int64_t N, in
   const char* wb = static_cast<const char*>(w);
   const char* arena = dc_.heap[dc_.sync.rank] + symm_off_;
   if (!(wb >= arena && wb + N * K * 2 <= arena + symm_bytes_)) return false;  // must be switch-visible in place
-  // 2 partial buffers (per source rank in peer-store mode) + W_avg prefetch
-  const int64_t need = (2 * (fused_wgrad_multicast() ? 1 : size()) + 1) * N * K * 2 + fused_wgrad_tiles(N, K) * 4 + 8192;
-  return wgrad_.count((N << 32) | K) > 0 || symm_cursor_ + need <= symm_bytes_;
+  // per shape: 2 partial buffers (per source rank in peer-store mode); per weight: its W_avg prefetch
+  const bool shape_known = wgrad_.count((N << 32) | K) > 0;
+  const bool weight_known = wgrad_avg_.count(wb - dc_.heap[dc_.sync.rank]) > 0;
+  if (shape_known && weight_known) return true;
+  int64_t need = 8192;
+  if (!shape_known) need += 2 * (fused_wgrad_multicast() ? 1 : size()) * N * K * 2 + fused_wgrad_tiles(N, K) * 4;
+  if (!weight_known) need += N * K * 2;
+  return symm_cursor_ + need <= symm_bytes_;
 }
 
 const void* CudaBackend::fused_wgrad_update(void* w, const void* dy, const void* x, int64_t Mb, int64_t N, int64_t K,
@@ -435,17 +440,18 @@ const void* CudaBackend::fused_wgrad_update(void* w, const void* dy, const void*
     it = wgrad_.emplace(key, st).first;  // the arena is zero-initialised: counters start at 0
   }
   FusedWgradState& st = it->second;
-  if (prefetch_avg && st.wavg_off < 0) st.wavg_off = symm_alloc(N * K * 2);  // same call sequence on every rank
-  chain(stream);
   const int64_t w_off = static_cast<const char*>(w) - dc_.heap[dc_.sync.rank];
+  int64_t& wavg_off = wgrad_avg_.emplace(w_off, -1).first->second;
+  if (prefetch_avg && wavg_off < 0) wavg_off = symm_alloc(N * K * 2);  // same call sequence on every rank
+  chain(stream);
   st.calls += 1;
   // per-call increments of the monotonic counters; the kernel multiplies by (device call index + 1)
   const uint32_t tile_target = static_cast<uint32_t>(fused_wgrad_signals_per_unit() * size());
   const uint32_t done_target = static_cast<uint32_t>(size() * fused_gemm_grid(dc_));
   launch_fused_wgrad_update(dc_, dy, x, Mb, N, K, ldy, ldx, w_off, st.stage_off, st.stage_stride, st.cnt_off,
-                            st.done_off, st.ksplit, tile_target, done_target, scale, prefetch_avg ? st.wavg_off : -1,
+                            st.done_off, st.ksplit, tile_target, done_target, scale, prefetch_avg ? wavg_off : -1,
                             stream, st.epoch_off, gscale, fused_wgrad_multicast(), st.src_stride);
-  return prefetch_avg ? symm_ptr(st.wavg_off) : nullptr;
+  return prefetch_avg ? symm_ptr(wavg_off) : nullptr;
 }
 
 // ---------------------------------------------------------------------------

@@ -152,12 +152,16 @@ class CudaBackend final : public Backend {
     uint64_t calls = 0;
   };
   std::unordered_map<int64_t, FusedLinearState> fused_;  // key = N << 32 | K
+  // staging and counters are shared by every weight of one shape (calls on one stream are sequential)
   struct FusedWgradState {
-    int64_t stage_off = 0, stage_stride = 0, src_stride = 0, cnt_off = 0, done_off = 0, wavg_off = -1, epoch_off = -1;
+    int64_t stage_off = 0, stage_stride = 0, src_stride = 0, cnt_off = 0, done_off = 0, epoch_off = -1;
     int ksplit = 1;
     uint64_t calls = 0;
   };
   std::unordered_map<int64_t, FusedWgradState> wgrad_;  // key = N << 32 | K
+  // prefetched average per WEIGHT (two layers of one shape must not share it): weight heap offset ->
+  // offset of its W_avg buffer, -1 until the first prefetching call
+  std::unordered_map<int64_t, int64_t> wgrad_avg_;
   int64_t symm_off_ = 0, symm_cursor_ = 0, symm_bytes_ = 0;
   int64_t p2p_ce_min_bytes_ = 2 << 20;  // copy-engine path threshold (M4T_P2P_CE_MIN_KB)
 };

@@ -4,5 +4,6 @@ examples/simple_linear_regression.py); BASELINE.json adds the 4096x4096
 data-parallel linear layer."""
 from .linear_regression import LinearRegression, make_regression_shard
 from .dp_linear import DPLinearModel
+from .dp_mlp import DPMLPModel
 
-__all__ = ["LinearRegression", "make_regression_shard", "DPLinearModel"]
+__all__ = ["LinearRegression", "make_regression_shard", "DPLinearModel", "DPMLPModel"]

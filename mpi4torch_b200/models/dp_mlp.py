@@ -1,0 +1,86 @@
+"""Data-parallel two-layer MLP: ``Linear(D, H) -> GELU(tanh) -> Linear(H, O)`` with biases and an MSE loss.
+
+One training step, every rank, on the autograd graph:
+
+    local = dp_mlp_mse(x, W1, b1, W2, b2, t)   bias+GELU GEMM -> bias+MSE GEMM (loss, dL/dy, bias-gradient partials)
+    loss  = comm.Allreduce(local, MPI_SUM)     the library's differentiable Allreduce
+    loss.backward()                            GELU-backward GEMM, the two wgrad GEMMs (with the SGD step and, with
+                                               more than one rank, the gradient reduce-scatter and the next step's
+                                               weight average inside them), column sums -> bias updates
+
+With ``sgd_in_backward=False`` (or off the kernel path) the parameters get ordinary ``.grad`` tensors and
+``train_step`` applies SGD.  Biases are fp32 when the weights are 16-bit: a bf16 bias would lose SGD updates
+below 2^-8 of its value.
+"""
+from __future__ import annotations
+
+import torch
+
+import mpi4torch_b200 as m4t
+from mpi4torch_b200.ops import InBackwardSGD, dp_mlp_mse, dp_mlp_mse_supported, mlp_in_backward_sgd_supported
+
+
+class DPMLPModel:
+    def __init__(self, in_features: int, hidden_features: int, out_features: int, comm=None, device="cuda",
+                 dtype=torch.bfloat16, lr: float = 1e-4, seed: int = 0, sgd_in_backward: bool = True,
+                 prefetch: bool = True):
+        self.comm = m4t.COMM_WORLD if comm is None else comm
+        g = torch.Generator().manual_seed(seed)  # identical initial parameters on every rank
+        w1 = torch.randn(hidden_features, in_features, generator=g) * (in_features ** -0.5)
+        w2 = torch.randn(out_features, hidden_features, generator=g) * (hidden_features ** -0.5)
+        dev = torch.device(device)
+        symmetric = (dev.type == "cuda" and dtype == torch.bfloat16 and self.comm.size > 1 and self.comm.is_world
+                     and m4t.cuda_backend_ready() and hasattr(torch.ops.mpi4torch_b200, "symmetric_empty"))
+        self.w1 = self._weight(w1, dev, dtype, symmetric)
+        self.w2 = self._weight(w2, dev, dtype, symmetric)
+        bias_dtype = torch.float32 if dtype in (torch.bfloat16, torch.float16) else dtype
+        self.b1 = torch.zeros(hidden_features, device=dev, dtype=bias_dtype, requires_grad=True)
+        self.b2 = torch.zeros(out_features, device=dev, dtype=bias_dtype, requires_grad=True)
+        self.lr = lr
+        self.sgd_in_backward = sgd_in_backward
+        self.optimizers = (InBackwardSGD(lr, prefetch=prefetch), InBackwardSGD(lr, prefetch=prefetch))
+        self._opt_ok = {}
+
+    @staticmethod
+    def _weight(w: torch.Tensor, dev: torch.device, dtype, symmetric: bool) -> torch.Tensor:
+        if symmetric:
+            # in the symmetric heap the fused backward kernels (and the NVSwitch) update it in place
+            storage = torch.ops.mpi4torch_b200.symmetric_empty(list(w.shape), dtype)
+            storage.copy_(w.to(dtype))
+            return storage.requires_grad_()
+        return w.to(device=dev, dtype=dtype).requires_grad_()
+
+    def parameters(self):
+        return [self.w1, self.b1, self.w2, self.b2]
+
+    def _in_backward(self, x: torch.Tensor, target: torch.Tensor) -> bool:
+        if not self.sgd_in_backward:
+            return False
+        key = (x.device, x.dtype, tuple(x.shape), tuple(x.stride()), tuple(target.shape))
+        ok = self._opt_ok.get(key)
+        if ok is None:
+            ok = (dp_mlp_mse_supported(x, self.w1, self.b1, self.w2, self.b2, target, self.comm)
+                  and mlp_in_backward_sgd_supported(x, self.w1, self.w2, self.comm))
+            self._opt_ok[key] = ok
+        return ok
+
+    def loss(self, x: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
+        """Global mean-squared-error loss as a differentiable one-element tensor."""
+        opts = self.optimizers if self._in_backward(x, target) else None
+        local = dp_mlp_mse(x, self.w1, self.b1, self.w2, self.b2, target, self.comm,
+                           loss_scale=1.0 / (x.shape[0] * self.comm.size), optimizers=opts)
+        return self.comm.Allreduce(local, m4t.MPI_SUM)
+
+    def train_step(self, x: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
+        """forward + backward + SGD update through the autograd graph; returns the (global) loss."""
+        value = self.loss(x, target)
+        value.backward()
+        if any(p.grad is not None for p in self.parameters()):  # the optimizers did not run inside backward
+            for opt in self.optimizers:
+                opt.invalidate()
+            with torch.no_grad():
+                for p in self.parameters():
+                    if p.grad is not None:
+                        p.add_(p.grad, alpha=-self.lr)
+                        p.grad = None
+        return value.detach().reshape(())

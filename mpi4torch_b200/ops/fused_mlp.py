@@ -1,0 +1,167 @@
+"""Data-parallel two-layer MLP (``Linear -> GELU(tanh) -> Linear``, biases, MSE loss) as one autograd node
+backed by the library's wgmma kernels.
+
+``dp_mlp_mse(x, W1, b1, W2, b2, t, ...)``  loss_local = loss_scale * sum((y - t)^2),
+    z = x @ mean_ranks(W1)^T + mean_ranks(b1),  h = gelu_tanh(z),  y = h @ mean_ranks(W2)^T + mean_ranks(b2)
+
+Forward is two GEMMs with their epilogues (csrc/kernels/gemm_wgmma.cu): bias + GELU storing z and h, then
+bias + MSE storing dL/dy, adding the loss and writing column-sum partials of dL/dy (y itself is never stored).
+Backward is the GELU-backward GEMM (dz, with its column-sum partials), the two weight-gradient GEMMs and the
+deterministic column-sum reduce for the biases.  With :class:`InBackwardSGD` optimizers the weights are
+updated inside backward by the wgrad kernels (with P > 1: reduce-scatter -> SGD -> multicast -> average of
+the new weights for the next forward, one kernel per weight) and the biases by ``allreduce_axpy_``; the
+parameters then receive no ``.grad``.
+
+Elsewhere (CPU tensors, other dtypes, shapes the kernels reject, communicators created by ``Split``) the same
+math runs as the composition ``F.linear -> F.gelu(tanh) -> F.linear -> MSE`` on ``AllreduceFused`` averages,
+which gives the same gradients.
+"""
+from __future__ import annotations
+
+from typing import Optional, Sequence
+
+import torch
+import torch.nn.functional as F
+
+import mpi4torch_b200 as m4t
+
+from .fused_linear import InBackwardSGD, _ops
+
+
+def _average(comm, p: torch.Tensor) -> torch.Tensor:
+    return p if comm.size == 1 else comm.AllreduceFused(p, m4t.MPI_SUM, 1.0 / comm.size, None)
+
+
+def _update_weight(ops, comm, opt: InBackwardSGD, weight, dy, x, g) -> None:
+    scale = -opt.lr / comm.size
+    if comm.size == 1:
+        ops.wgrad_sgd_(weight, dy, x, scale, g)
+        opt.remember(weight, None)
+    elif opt.prefetch:
+        opt.remember(weight, ops.wgrad_allreduce_sgd_prefetch_(weight, dy, x, scale, g))
+    else:
+        ops.wgrad_allreduce_sgd_(weight, dy, x, scale, g)
+        opt.remember(weight, None)
+
+
+class _DPMLPMSE(torch.autograd.Function):
+    """Local MSE loss of the data-parallel two-layer MLP; backward folds the upstream device scalar ``g``
+    into the kernels' epilogues (never read on the host)."""
+
+    @staticmethod
+    def forward(ctx, x, w1, b1, w2, b2, target, comm_holder, loss_scale, opts):
+        comm = comm_holder[0]
+        ops = _ops()
+        w1_avg = opts[0].take_prefetched(w1) if opts is not None else None
+        w2_avg = opts[1].take_prefetched(w2) if opts is not None else None
+        w1_avg = _average(comm, w1) if w1_avg is None else w1_avg
+        w2_avg = _average(comm, w2) if w2_avg is None else w2_avg
+        h, z = ops.linear_bias_gelu_forward(x, w1_avg, _average(comm, b1))
+        dy, local, dy_part = ops.linear_bias_mse_forward_local(h, w2_avg, _average(comm, b2), target, loss_scale,
+                                                                2.0 * loss_scale)
+        ctx.save_for_backward(x, h, z, dy, w1_avg, w2_avg, dy_part)
+        ctx.comm, ctx.opts, ctx.params = comm, opts, (w1, b1, w2, b2)
+        return local
+
+    @staticmethod
+    def backward(ctx, g):
+        x, h, z, dy, w1_avg, w2_avg, dy_part = ctx.saved_tensors
+        comm, opts = ctx.comm, ctx.opts
+        w1, b1, w2, b2 = ctx.params
+        ops = _ops()
+        g = g.reshape(1).to(torch.float32)
+        need = ctx.needs_input_grad
+        # Order of the reads and updates.  Every read of a layer's averaged weight is enqueued before that
+        # layer's fused update, which may overwrite it: at P = 1 the average IS the weight (wgrad_sgd_ updates it
+        # in place), and with a prefetching optimizer it is the buffer the update kernel refills with the next
+        # average.  Across ranks this needs no copy either: the update kernel writes the new average of a tile
+        # into a peer's buffer only after every rank's partial gradients of that tile have arrived, and a rank
+        # produces its partials only after its own earlier reads, which come first in its stream.
+        #   1. dz reads W2_avg;  2. layer-2 update;  3. dx reads W1_avg;  4. layer-1 update;  5. biases.
+        dz, dz_part = ops.gemm_nn_gelu_backward(dy, w2_avg, z, g)
+        gx = gw1 = gb1 = gw2 = gb2 = None
+        if opts is not None:
+            _update_weight(ops, comm, opts[1], w2, dy, h, g)
+        elif need[3]:
+            gw2 = comm.AllreduceFused(ops.wgrad_bf16(dy, h, g), m4t.MPI_SUM, 1.0 / comm.size, None)
+        if need[0]:
+            gx = ops.gemm_bf16_nn(dz, w1_avg)
+        if opts is not None:
+            _update_weight(ops, comm, opts[0], w1, dz, x, None)
+        elif need[1]:
+            gw1 = comm.AllreduceFused(ops.wgrad_bf16(dz, x, None), m4t.MPI_SUM, 1.0 / comm.size, None)
+        db2 = ops.column_sum(dy_part, g)
+        db1 = ops.column_sum(dz_part, None)
+        if opts is not None:
+            # one path for every P, summed in a fixed order: the biases stay bit-identical across ranks
+            ops.allreduce_axpy_(b2, db2, -opts[1].lr / comm.size)
+            ops.allreduce_axpy_(b1, db1, -opts[0].lr / comm.size)
+        else:
+            if need[4]:
+                gb2 = comm.AllreduceFused(db2, m4t.MPI_SUM, 1.0 / comm.size, None)
+            if need[2]:
+                gb1 = comm.AllreduceFused(db1, m4t.MPI_SUM, 1.0 / comm.size, None)
+        return gx, gw1, gb1, gw2, gb2, None, None, None, None
+
+
+def _kernel_ops_present() -> bool:
+    return hasattr(_ops(), "linear_bias_gelu_forward")
+
+
+def dp_mlp_mse_supported(x: torch.Tensor, w1: torch.Tensor, b1: torch.Tensor, w2: torch.Tensor, b2: torch.Tensor,
+                         target: torch.Tensor, comm=None) -> bool:
+    """Does :func:`dp_mlp_mse` run on the library's kernels for these tensors (plain-gradient mode)?
+    D, H, O must be multiples of 128 and the batch a multiple of 64."""
+    c = m4t.COMM_WORLD if comm is None else comm
+    if not (c.is_world and m4t.cuda_backend_ready() and _kernel_ops_present()):
+        return False
+    ts = (x, w1, w2, target)
+    if not all(t.is_cuda and t.dim() == 2 and t.dtype == torch.bfloat16 and t.is_contiguous() for t in ts):
+        return False
+    if not all(b.is_cuda and b.dim() == 1 and b.dtype == torch.float32 and b.is_contiguous() for b in (b1, b2)):
+        return False
+    (B, D), (H, D1), (O, H1) = x.shape, w1.shape, w2.shape
+    if not (D1 == D and H1 == H and b1.shape[0] == H and b2.shape[0] == O and tuple(target.shape) == (B, O)):
+        return False
+    return B % 64 == 0 and D % 128 == 0 and H % 128 == 0 and O % 128 == 0 and B > 0
+
+
+def mlp_in_backward_sgd_supported(x: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, comm=None) -> bool:
+    """Can backward update both weights inside their wgrad kernels?  With P > 1 the weights must come from
+    ``symmetric_empty()``, D, H, O must be multiples of 256, the batch a multiple of 128, and the arena must
+    have room for both weights' buffers."""
+    c = m4t.COMM_WORLD if comm is None else comm
+    B = x.shape[0]
+    h_like = x.new_empty((B, w1.shape[0]))
+    dy_like = x.new_empty((B, w2.shape[0]))
+    if c.size == 1:
+        return bool(_ops().wgrad_bf16_supported(h_like, x) and _ops().wgrad_bf16_supported(dy_like, h_like))
+    return bool(_ops().wgrad_allreduce_sgd_supported(w1, h_like, x)
+                and _ops().wgrad_allreduce_sgd_supported(w2, dy_like, h_like))
+
+
+def dp_mlp_mse(x: torch.Tensor, w1: torch.Tensor, b1: torch.Tensor, w2: torch.Tensor, b2: torch.Tensor,
+               target: torch.Tensor, comm=None, *, loss_scale: float,
+               optimizers: Optional[Sequence[InBackwardSGD]] = None) -> torch.Tensor:
+    """``loss_scale * sum((MLP(x) - target)^2)`` of THIS rank's batch as a differentiable one-element fp32
+    tensor, with every parameter averaged over ranks; sum it over ranks with ``comm.Allreduce``.
+
+    ``optimizers``: ``(opt1, opt2)``, one :class:`InBackwardSGD` per layer, makes ``backward`` apply the SGD
+    step to ``(w1, b1)`` and ``(w2, b2)`` itself; the parameters then receive no ``.grad``."""
+    c = m4t.COMM_WORLD if comm is None else comm
+    if dp_mlp_mse_supported(x, w1, b1, w2, b2, target, c):
+        if optimizers is not None:
+            if len(optimizers) != 2:
+                raise ValueError("mpi4torch_b200: dp_mlp_mse takes one InBackwardSGD per layer")
+            if not mlp_in_backward_sgd_supported(x, w1, w2, c):
+                raise RuntimeError("mpi4torch_b200: InBackwardSGD for the MLP needs, with more than one rank, bf16 weights "
+                                   "from symmetric_empty() with D, H, O % 256 == 0 and batch % 128 == 0")
+            optimizers = tuple(optimizers)
+        return _DPMLPMSE.apply(x, w1, b1, w2, b2, target, [c], float(loss_scale), optimizers)
+    if optimizers is not None:
+        raise RuntimeError("mpi4torch_b200: InBackwardSGD is only available on the CUDA kernel path")
+    avg = lambda p: c.AllreduceFused(p, m4t.MPI_SUM, 1.0 / c.size, None)  # noqa: E731
+    acc = torch.float64 if x.dtype == torch.float64 else torch.float32  # accumulate in fp32 (fp64 inputs stay fp64)
+    h = F.gelu(F.linear(x, avg(w1), avg(b1).to(x.dtype)), approximate="tanh")
+    y = F.linear(h, avg(w2), avg(b2).to(h.dtype))
+    return ((y.to(acc) - target.to(acc)).square().sum() * loss_scale).reshape(1)
