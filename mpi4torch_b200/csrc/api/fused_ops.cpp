@@ -68,9 +68,19 @@ Tensor gemm_bf16_nn(const Tensor& a, const Tensor& b) {
   return y;
 }
 
-bool gemm_bf16_tn_ok(const Tensor& x, const Tensor& w) {
+// Also answers for the epilogue operands when given: an MSE target [M, N] (bf16) and a bias [N] (fp32).
+bool gemm_bf16_tn_ok(const Tensor& x, const Tensor& w, const c10::optional<Tensor>& target,
+                     const c10::optional<Tensor>& bias) {
   if (!(x.is_cuda() && w.is_cuda() && x.dim() == 2 && w.dim() == 2 && x.scalar_type() == at::kBFloat16 &&
         w.scalar_type() == at::kBFloat16 && x.stride(1) == 1 && w.stride(1) == 1 && x.size(1) == w.size(1)))
+    return false;
+  if (target.has_value() &&
+      !(target->is_cuda() && target->dim() == 2 && target->scalar_type() == at::kBFloat16 && target->stride(1) == 1 &&
+        target->size(0) == x.size(0) && target->size(1) == w.size(0) &&
+        epilogue_bf16_pairs_ok(target->data_ptr(), target->stride(0))))
+    return false;
+  if (bias.has_value() && !(bias->is_cuda() && bias->dim() == 1 && bias->scalar_type() == at::kFloat &&
+                            bias->is_contiguous() && bias->size(0) == w.size(0) && epilogue_bias_ok(bias->data_ptr<float>())))
     return false;
   return World::instance().cuda_ready() &&
          gemm_bf16_tn_supported(x.size(0), w.size(0), x.size(1), x.data_ptr(), w.data_ptr(), x.data_ptr(), x.stride(0),
@@ -112,6 +122,9 @@ std::tuple<Tensor, Tensor, Tensor> linear_mse_forward(const Tensor& x, const Ten
   check_2d_bf16(target, "target");
   TORCH_CHECK(x.size(1) == w.size(1) && target.size(0) == x.size(0) && target.size(1) == w.size(0),
               "mpi4torch_b200: linear_mse_forward shape mismatch");
+  // checked here as well as in the GEMM launchers: with more than one rank a weight average is launched first
+  TORCH_CHECK(epilogue_bf16_pairs_ok(target.data_ptr(), target.stride(0)),
+              "mpi4torch_b200: the MSE target needs a 4-byte-aligned base and an even row stride");
   c10::cuda::CUDAGuard guard(x.device());
   cudaStream_t stream = c10::cuda::getCurrentCUDAStream(x.device().index()).stream();
   Tensor dy = at::empty({x.size(0), w.size(0)}, x.options());
@@ -397,7 +410,7 @@ TORCH_LIBRARY_FRAGMENT(mpi4torch_b200, m) {
   m.def("gemm_bf16_tn(Tensor x, Tensor w) -> Tensor", &gemm_bf16_tn);
   m.def("gemm_bf16_nn(Tensor a, Tensor b) -> Tensor", &gemm_bf16_nn);
   m.def("gemm_bf16_nn_supported(Tensor a, Tensor b) -> bool", &gemm_bf16_nn_ok);
-  m.def("gemm_bf16_tn_supported(Tensor x, Tensor w) -> bool", &gemm_bf16_tn_ok);
+  m.def("gemm_bf16_tn_supported(Tensor x, Tensor w, Tensor? target=None, Tensor? bias=None) -> bool", &gemm_bf16_tn_ok);
   m.def("allreduce_linear_supported(Tensor x, Tensor w) -> bool", &allreduce_linear_supported);
   m.def("allreduce_linear_fused(Tensor x, Tensor w, float scale) -> (Tensor, Tensor)", &allreduce_linear_fused);
 }

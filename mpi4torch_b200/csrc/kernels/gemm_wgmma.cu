@@ -345,12 +345,21 @@ bool gemm_bf16_tn_supported(int64_t M, int64_t N, int64_t K, const void* A, cons
                             int64_t ldb, int64_t ldc) {
   auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
   return M > 0 && N > 0 && K > 0 && (K % 8) == 0 && (N % 8) == 0 && (lda % 8) == 0 && (ldb % 8) == 0 && (ldc % 8) == 0 &&
-         al16(A) && al16(B) && al16(C) && M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31);
+         lda >= K && ldb >= K && ldc >= N && al16(A) && al16(B) && al16(C) && M < (1ll << 31) && N < (1ll << 31) &&
+         K < (1ll << 31);
 }
+
+bool epilogue_bf16_pairs_ok(const void* p, int64_t ld) {
+  return (reinterpret_cast<uintptr_t>(p) & 3u) == 0 && ld % 2 == 0 && ld >= 0 && ld < (1ll << 31);
+}
+
+bool epilogue_bias_ok(const float* bias) { return (reinterpret_cast<uintptr_t>(bias) & 7u) == 0; }
 
 void launch_gemm_bf16_tn(const void* A, const void* B, void* C, int64_t M, int64_t N, int64_t K, int64_t lda,
                          int64_t ldb, int64_t ldc, int sm_count, cudaStream_t stream, const MseEpilogue* mse) {
   M4T_CHECK(gemm_bf16_tn_supported(M, N, K, A, B, C, lda, ldb, ldc), "unsupported GEMM shape/alignment for the wgmma path");
+  M4T_CHECK(mse == nullptr || epilogue_bf16_pairs_ok(mse->target, mse->ldt),
+            "the MSE target needs a 4-byte-aligned base and an even row stride");
   constexpr int BN = tile_n<false>();
   const CUtensorMap ta = make_tmap(A, M, K, lda, BM);
   const CUtensorMap tb = make_tmap(B, N, K, ldb, BN);
@@ -407,6 +416,8 @@ void launch_fused_allreduce_gemm(const DeviceComm& dc, const void* x, void* y, i
             "fused Allreduce->GEMM: N must be a multiple of 256 and 256 % ranks == 0");
   const char* wavg = dc.heap[dc.sync.rank] + wavg_off;
   M4T_CHECK(gemm_bf16_tn_supported(M, N, K, x, wavg, y, ldx, K, ldy), "unsupported GEMM shape/alignment for the fused path");
+  M4T_CHECK(mse == nullptr || epilogue_bf16_pairs_ok(mse->target, mse->ldt),
+            "the MSE target needs a 4-byte-aligned base and an even row stride");
   constexpr int BN = tile_n<true>();
   const CUtensorMap ta = make_tmap(x, M, K, ldx, BM);
   const CUtensorMap tb = make_tmap(wavg, N, K, K, BN);
@@ -446,6 +457,7 @@ void launch_gemm_bias_gelu(const void* A, const void* B, const float* bias, void
                            int64_t K, int64_t lda, int64_t ldb, int64_t ldc, int sm_count, cudaStream_t stream) {
   M4T_CHECK(gemm_bf16_tn_supported(M, N, K, A, B, z, lda, ldb, ldc) && (reinterpret_cast<uintptr_t>(h) & 15u) == 0,
             "unsupported GEMM shape/alignment for the wgmma bias+GELU path");
+  M4T_CHECK(epilogue_bias_ok(bias), "the bias needs an 8-byte-aligned base");
   MlpEpiArgs e{};
   e.bias = bias;
   e.h_out = h;
@@ -457,6 +469,8 @@ void launch_gemm_bias_mse_colsum(const void* A, const void* B, const float* bias
                                  int64_t N, int64_t K, int64_t lda, int64_t ldb, int64_t ldc, int sm_count,
                                  cudaStream_t stream, const MseEpilogue& mse) {
   M4T_CHECK(gemm_bf16_tn_supported(M, N, K, A, B, dy, lda, ldb, ldc), "unsupported GEMM shape/alignment for the wgmma bias+MSE path");
+  M4T_CHECK(epilogue_bf16_pairs_ok(mse.target, mse.ldt), "the MSE target needs a 4-byte-aligned base and an even row stride");
+  M4T_CHECK(epilogue_bias_ok(bias), "the bias needs an 8-byte-aligned base");
   GemmArgs g = plain_args(dy, M, N, K, ldc);
   set_mse(g, &mse);
   MlpEpiArgs e{};
@@ -469,8 +483,9 @@ void launch_gemm_bias_mse_colsum(const void* A, const void* B, const float* bias
 void launch_gemm_nn_gelu_bwd_colsum(const void* A, const void* B, const void* z, void* dz, float* colsum, int64_t M,
                                     int64_t N, int64_t K, int64_t lda, int64_t ldb, int64_t ldz, int64_t ldc,
                                     int sm_count, cudaStream_t stream, const float* gscale) {
-  M4T_CHECK(gemm_bf16_nn_supported(M, N, K, A, B, dz, lda, ldb, ldc) && ldz % 2 == 0,
+  M4T_CHECK(gemm_bf16_nn_supported(M, N, K, A, B, dz, lda, ldb, ldc),
             "unsupported GEMM shape/alignment for the wgmma GELU-backward path");
+  M4T_CHECK(epilogue_bf16_pairs_ok(z, ldz), "z needs a 4-byte-aligned base and an even row stride");
   GemmArgs g = plain_args(dz, M, N, K, ldc);
   g.T = z;
   g.ldt = static_cast<int>(ldz);

@@ -115,6 +115,11 @@ struct MseEpilogue {
   float* loss_acc;
   float loss_scale, grad_scale;
 };
+// Operands the GEMM epilogues read with vector loads.  The MSE target and the GELU input z are read as bf16 pairs
+// (4 bytes at an even column): they need a 4-byte-aligned base and an even leading dimension.  The bias is read as
+// fp32 pairs: it needs an 8-byte-aligned base.  The launchers check both before launching.
+bool epilogue_bf16_pairs_ok(const void* p, int64_t ld);
+bool epilogue_bias_ok(const float* bias);
 // C[M,N] = A[M,K] * B[N,K]^T, bf16 in / fp32 accumulate / bf16 out.
 void launch_gemm_bf16_tn(const void* A, const void* B, void* C, int64_t M, int64_t N, int64_t K, int64_t lda,
                          int64_t ldb, int64_t ldc, int sm_count, cudaStream_t stream, const MseEpilogue* mse = nullptr);

@@ -190,7 +190,7 @@ def dp_linear_mse_supported(x: torch.Tensor, weight: torch.Tensor, target: torch
             and target.dtype == torch.bfloat16 and weight.dtype == torch.bfloat16 and weight.is_cuda
             and x.stride(1) == 1 and target.stride(1) == 1 and weight.is_contiguous()
             and m4t.cuda_backend_ready() and hasattr(_ops(), "linear_mse_forward")
-            and _ops().gemm_bf16_tn_supported(x, weight))
+            and _ops().gemm_bf16_tn_supported(x, weight, target))
 
 
 def in_backward_sgd_supported(x: torch.Tensor, weight: torch.Tensor, comm) -> bool:

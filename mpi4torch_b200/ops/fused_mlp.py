@@ -111,7 +111,8 @@ def _kernel_ops_present() -> bool:
 def dp_mlp_mse_supported(x: torch.Tensor, w1: torch.Tensor, b1: torch.Tensor, w2: torch.Tensor, b2: torch.Tensor,
                          target: torch.Tensor, comm=None) -> bool:
     """Does :func:`dp_mlp_mse` run on the library's kernels for these tensors (plain-gradient mode)?
-    D, H, O must be multiples of 128 and the batch a multiple of 64."""
+    D, H, O must be multiples of 128, the batch a multiple of 64, and every operand aligned as the kernels read
+    it (see ``gemm_bf16_tn_supported``)."""
     c = m4t.COMM_WORLD if comm is None else comm
     if not (c.is_world and m4t.cuda_backend_ready() and _kernel_ops_present()):
         return False
@@ -123,7 +124,12 @@ def dp_mlp_mse_supported(x: torch.Tensor, w1: torch.Tensor, b1: torch.Tensor, w2
     (B, D), (H, D1), (O, H1) = x.shape, w1.shape, w2.shape
     if not (D1 == D and H1 == H and b1.shape[0] == H and b2.shape[0] == O and tuple(target.shape) == (B, O)):
         return False
-    return B % 64 == 0 and D % 128 == 0 and H % 128 == 0 and O % 128 == 0 and B > 0
+    if not (B % 64 == 0 and D % 128 == 0 and H % 128 == 0 and O % 128 == 0 and B > 0):
+        return False
+    # base alignment and row strides of every operand the two forward GEMMs read (h is allocated by the first)
+    ops = _ops()
+    return bool(ops.gemm_bf16_tn_supported(x, w1, None, b1)
+                and ops.gemm_bf16_tn_supported(x.new_empty((B, H)), w2, target, b2))
 
 
 def mlp_in_backward_sgd_supported(x: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, comm=None) -> bool:
