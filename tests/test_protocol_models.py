@@ -1,8 +1,10 @@
 """Pure-Python mirrors of the index arithmetic of the fused backward kernel
-(csrc/kernels/wgrad_wgmma.cu).  They cannot check the memory model, but they do
+(csrc/kernels/wgrad_wgmma.cu) and of the smem ring shared by the wgmma kernels
+(csrc/kernels/wgmma_pipeline.cuh).  They cannot check the memory model, but they do
 check what is easy to get wrong in a persistent, role-split kernel: that the work
-distribution covers every element exactly once and that the counters reach exactly the
-targets the host computes (csrc/runtime/cuda_backend.cpp::fused_wgrad_update)."""
+distribution covers every element exactly once, that the counters reach exactly the
+targets the host computes (csrc/runtime/cuda_backend.cpp::fused_wgrad_update), and that
+every mbarrier wait is on a phase that some arrival completes."""
 import itertools
 
 import numpy as np
@@ -330,3 +332,176 @@ def test_push_epilogue_box_coordinates_cover_the_staging_area_once():
         for h in range(ksplit):
             blk = area[h * N + n_blk * BM:h * N + (n_blk + 1) * BM, k_blk * BN:(k_blk + 1) * BN]
             assert (blk == (1 if h < parts else 0)).all(), (t, h)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# The smem ring of the single-GPU GEMM and wgrad kernels (csrc/kernels/wgmma_pipeline.cuh, gemm_wgmma.cu)
+# ---------------------------------------------------------------------------------------------------------------
+GEMM_BM, GEMM_BN, GEMM_BK = 128, 256, 64
+RING_STAGES = 4        # Tile<256>::kStages
+CONSUMER_WARPS = 8     # kConsumerWarps: lane 0 of every consumer warp arrives on `empty`
+
+
+class _MBarrier:
+    """An mbarrier: `count` arrivals complete the current phase.  try_wait.parity(p) succeeds once the phase of
+    parity p has completed, i.e. while the current (incomplete) phase has the other parity."""
+
+    def __init__(self, count):
+        self.count, self.pending, self.completed = count, count, 0
+
+    def arrive(self):
+        assert self.pending > 0
+        self.pending -= 1
+        if self.pending == 0:
+            self.completed += 1
+            self.pending = self.count
+
+    def passes(self, parity):
+        return (self.completed & 1) != parity
+
+
+def _advance(stage, phase):
+    stage += 1
+    return (0, phase ^ 1) if stage == RING_STAGES else (stage, phase)
+
+
+def simulate_ring(tiles, seed):
+    """One CTA: `tiles` is its list of (tile id, k_blocks) in loop order.  The producer runs load_stage for every
+    k-block, each consumer warp runs mma_tile (it hands stage kb back only after the MMAs of kb + 1 are issued,
+    and its last stage after the tile).  Agents interleave at random; every wait must be satisfiable.  Returns the
+    producer's (stage, parity) sequence, each warp's sequence and the tiles each warp finished."""
+    import random
+
+    rng = random.Random(seed)
+    full = [_MBarrier(1) for _ in range(RING_STAGES)]
+    empty = [_MBarrier(CONSUMER_WARPS) for _ in range(RING_STAGES)]
+    content = [None] * RING_STAGES
+    held = [set() for _ in range(CONSUMER_WARPS)]  # stages a warp's in-flight MMAs still read
+    fills = [0] * RING_STAGES
+    prod_seq, warp_seq, done = [], [[] for _ in range(CONSUMER_WARPS)], [[] for _ in range(CONSUMER_WARPS)]
+
+    def producer():
+        stage, phase = 0, 0
+        for t, kbs in tiles:
+            for kb in range(kbs):
+                f = fills[stage]
+                yield empty[stage], phase ^ 1, f  # load_stage: wait until the f previous uses were released
+                assert not any(stage in h for h in held), "TMA overwrote a stage an MMA still reads"
+                content[stage] = (t, kb)
+                fills[stage] += 1
+                prod_seq.append((stage, phase))
+                full[stage].arrive()  # arrive_expect_tx + the bytes landing
+                stage, phase = _advance(stage, phase)
+
+    def consumer(w):
+        stage, phase, use = 0, 0, [0] * RING_STAGES
+        for t, kbs in tiles:
+            prev = None
+            for kb in range(kbs):
+                yield full[stage], phase, use[stage] + 1
+                assert content[stage] == (t, kb), f"warp {w} read {content[stage]} for {(t, kb)}"
+                use[stage] += 1
+                held[w].add(stage)
+                warp_seq[w].append((stage, phase))
+                yield None  # the MMAs of this k-block are issued; wait_group 1 retires the previous ones
+                if prev is not None:
+                    held[w].discard(prev)
+                    empty[prev].arrive()
+                prev = stage
+                stage, phase = _advance(stage, phase)
+            held[w].discard(prev)  # wait_group 0, then the last stage goes back
+            empty[prev].arrive()
+            done[w].append(t)
+
+    agents = [producer()] + [consumer(w) for w in range(CONSUMER_WARPS)]
+    waits = [None] * len(agents)
+    live = set(range(len(agents)))
+    while live:
+        ready = [a for a in live if waits[a] is None or waits[a][0].passes(waits[a][1])]
+        assert ready, "deadlock: a wait on a parity that no arrival completes"
+        a = rng.choice(ready)
+        if waits[a] is not None:
+            bar, _, phases = waits[a]
+            assert bar.completed == phases, "a parity wait passed on the wrong phase (ABA)"
+        try:
+            waits[a] = next(agents[a])
+        except StopIteration:
+            live.discard(a)
+            waits[a] = None
+    return prod_seq, warp_seq, done
+
+
+def gemm_cta_tiles(M, N, K, grid):
+    """Tile loop of gemm_bf16_wgmma_kernel: CTA c takes tiles c, c + grid, ...; every tile has ceil(K / 64) k-blocks."""
+    tiles = -(-M // GEMM_BM) * -(-N // GEMM_BN)
+    kbs = -(-K // GEMM_BK)
+    return [[(t, kbs) for t in range(c, tiles, grid)] for c in range(grid)], tiles
+
+
+def ring_starts(cta_tiles):
+    """(stage, parity) at which each tile of one CTA starts."""
+    stage, phase, out = 0, 0, []
+    for _, kbs in cta_tiles:
+        out.append((stage, phase))
+        for _ in range(kbs):
+            stage, phase = _advance(stage, phase)
+    return out
+
+
+@pytest.mark.parametrize("M,N,K,grid", [(300, 520, 328, 3), (129, 264, 200, 2), (1, 8, 8, 1), (257, 520, 72, 5),
+                                        (640, 512, 1000, 7), (256, 256, 64, 1)])
+def test_gemm_ring_covers_every_tile_and_matches_parities(M, N, K, grid):
+    per_cta, tiles = gemm_cta_tiles(M, N, K, min(grid, -(-M // GEMM_BM) * -(-N // GEMM_BN)))
+    finished = []
+    for c, cta_tiles in enumerate(per_cta):
+        for seed in range(3):
+            prod_seq, warp_seq, done = simulate_ring(cta_tiles, seed=c * 10 + seed)
+            assert len(prod_seq) == sum(kbs for _, kbs in cta_tiles)
+            for w in range(CONSUMER_WARPS):
+                assert warp_seq[w] == prod_seq, "a consumer waited on a (stage, parity) out of the producer's order"
+                assert done[w] == [t for t, _ in cta_tiles]
+        finished += [t for t, _ in cta_tiles]
+    assert sorted(finished) == list(range(tiles)), "a tile is computed twice or never"
+
+
+def test_wgrad_ring_with_split_units():
+    """wgrad_bf16_wgmma_kernel runs the same ring over work units of full or half batch depth (ksplit = 2)."""
+    for cta_units in ([(0, 6), (5, 3), (9, 3)], [(1, 5), (2, 5), (3, 1)], [(4, 1)] * 9):
+        prod_seq, warp_seq, _ = simulate_ring(cta_units, seed=len(cta_units))
+        assert all(s == prod_seq for s in warp_seq)
+
+
+def test_exact_arithmetic_sweep_starts_tiles_mid_ring():
+    """Why the wave sweep of test_gpu_exact_arithmetic.py uses 3 and 5 k-blocks per tile: with them, every CTA that
+    runs a second tile starts it at a non-zero stage of the 4-stage ring, and with 5 also on the flipped parity.
+    The multi-wave shapes of the tolerance tests (4096 -> 64 and 1000 -> 16 k-blocks) always start at stage 0."""
+    from test_gpu_exact_arithmetic import WAVE_KBLOCKS, gemm_wave_shape, wave_tile_counts, wgrad_wave_shape
+
+    for S in (132, 114):  # H100 SXM, H100 PCIe
+        for T in wave_tile_counts(S):
+            for kbs in WAVE_KBLOCKS:
+                M, N, K = gemm_wave_shape(T, kbs)
+                per_cta, tiles = gemm_cta_tiles(M, N, K, min(T, S))
+                assert tiles == T
+                assert all(c for c in per_cta)  # the grid is capped at the tile count: no CTA idles
+                assert sum(len(c) >= 2 for c in per_cta) == min(S, max(0, T - S))
+                for c in per_cta:
+                    starts = ring_starts(c)
+                    assert starts[0] == (0, 0)
+                    if len(c) >= 2:
+                        assert starts[1][0] != 0
+                        assert starts[1] == ((kbs % RING_STAGES), kbs // RING_STAGES)
+                if T == 2 * S + 1:  # one CTA runs a third tile, the last wave of a single tile
+                    assert sorted(len(c) for c in per_cta)[-2:] == [2, 3]
+            for kbs in (1, 3, 5):
+                Mb, Nw, Kw = wgrad_wave_shape(T, kbs)
+                assert (Nw // 128) * -(-Kw // 256) == T and Mb == 64 * kbs
+        for kbs in (16, 64):
+            for c in gemm_cta_tiles(8192, 4096, 64 * kbs, S)[0]:
+                assert all(s == (0, 0) for s in ring_starts(c))
+    # the whole sweep replays without deadlock through the ring model (one CTA per distinct tile list)
+    for kbs in WAVE_KBLOCKS:
+        per_cta, _ = gemm_cta_tiles(*gemm_wave_shape(2 * 132 + 1, kbs), 132)
+        for c in (per_cta[0], per_cta[-1]):
+            prod_seq, warp_seq, _ = simulate_ring(c, seed=kbs)
+            assert all(s == prod_seq for s in warp_seq)
