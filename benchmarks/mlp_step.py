@@ -5,6 +5,10 @@ epilogue kernel against its plain counterpart on the same shape.  One process; t
 with device events.  Prints one JSON line.
 
     python benchmarks/mlp_step.py [--batch 8192 --d 4096 --h 16384 --o 4096 --steps 20 --warmup 5 --reps 3]
+
+``--loss cross_entropy`` times DPMLPClassifier (softmax cross-entropy over O classes) against the eager composition
+with ``F.cross_entropy``, ``gemm_bias_xent`` against ``gemm_bf16_tn``, and ``xent_finish`` alone (as the whole
+cross-entropy op minus its GEMM), with the bytes xent_finish moves.
 """
 import argparse
 import json
@@ -19,7 +23,7 @@ import torch.nn.functional as F
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import mpi4torch_b200 as m4t  # noqa: E402
-from mpi4torch_b200.models import DPMLPModel  # noqa: E402
+from mpi4torch_b200.models import DPMLPClassifier, DPMLPModel  # noqa: E402
 from mpi4torch_b200.utils.timing import ClockSampler  # noqa: E402
 
 
@@ -53,6 +57,7 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--reps", type=int, default=3, help="alternations of the arms; medians are reported")
+    ap.add_argument("--loss", choices=("mse", "cross_entropy"), default="mse")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("mlp_step.py needs a GPU")
@@ -66,7 +71,12 @@ def main():
     t = torch.randn(B, O, device="cuda", generator=g).to(torch.bfloat16)
     lr = 1e-4
 
-    model = DPMLPModel(D, H, O, comm, device="cuda", lr=lr, seed=0)
+    xent = args.loss == "cross_entropy"
+    if xent:
+        t = torch.randint(0, O, (B,), device="cuda", generator=g)
+        model = DPMLPClassifier(D, H, O, comm, device="cuda", lr=lr, seed=0)
+    else:
+        model = DPMLPModel(D, H, O, comm, device="cuda", lr=lr, seed=0)
     if not model._in_backward(x, t):
         raise SystemExit(f"shape {(B, D, H, O)} is off the MLP kernel path")
 
@@ -76,7 +86,7 @@ def main():
 
     def eager_step():
         y = lin2(F.gelu(lin1(x), approximate="tanh"))
-        loss = (y.float() - t.float()).square().mean()
+        loss = F.cross_entropy(y.float(), t) if xent else (y.float() - t.float()).square().mean()
         loss.backward()
         with torch.no_grad():
             grads = [p.grad for p in eager_params]
@@ -88,11 +98,18 @@ def main():
     w1, b1 = model.w1.detach(), model.b1.detach()
     w2, b2 = model.w2.detach(), model.b2.detach()
     h, z = ops.linear_bias_gelu_forward(x, w1, b1)
-    dy, _, _ = ops.linear_bias_mse_forward_local(h, w2, b2, t, 1.0 / B, 2.0 / B)
+    if xent:
+        dy, _, _ = ops.linear_bias_xent_forward_local(h, w2, b2, t, 1.0 / B, 1.0 / B)
+        # the whole op (gemm_bias_xent, then xent_finish) against the plain GEMM; xent_kernel_times splits it
+        out_pair = {"gemm_bias_xent+xent_finish": (lambda: ops.linear_bias_xent_forward_local(h, w2, b2, t, 1.0 / B, 1.0 / B),
+                                                   lambda: ops.gemm_bf16_tn(h, w2))}
+    else:
+        dy, _, _ = ops.linear_bias_mse_forward_local(h, w2, b2, t, 1.0 / B, 2.0 / B)
+        out_pair = {"gemm_bias_mse_colsum": (lambda: ops.linear_bias_mse_forward_local(h, w2, b2, t, 1.0 / B, 2.0 / B),
+                                             lambda: ops.linear_mse_forward_local(h, w2, t, 1.0 / B, 2.0 / B))}
     pairs = {
         "gemm_bias_gelu": (lambda: ops.linear_bias_gelu_forward(x, w1, b1), lambda: ops.gemm_bf16_tn(x, w1)),
-        "gemm_bias_mse_colsum": (lambda: ops.linear_bias_mse_forward_local(h, w2, b2, t, 1.0 / B, 2.0 / B),
-                                 lambda: ops.linear_mse_forward_local(h, w2, t, 1.0 / B, 2.0 / B)),
+        **out_pair,
         "gemm_nn_gelu_bwd_colsum": (lambda: ops.gemm_nn_gelu_backward(dy, w2, z), lambda: ops.gemm_bf16_nn(dy, w2)),
     }
 
@@ -100,6 +117,10 @@ def main():
     for name, (new, plain) in pairs.items():
         arms[name] = new
         arms[name + ":plain"] = plain
+    if xent:  # the MSE step of the same shape, alternated with the others
+        mse_model = DPMLPModel(D, H, O, comm, device="cuda", lr=lr, seed=0)
+        t_mse = torch.randn(B, O, device="cuda", generator=g).to(torch.bfloat16)
+        arms["mse_model"] = lambda: mse_model.train_step(x, t_mse)
     for fn in arms.values():  # warm every shape: module loading, allocator, cuBLAS heuristics
         for _ in range(args.warmup):
             fn()
@@ -133,7 +154,41 @@ def main():
         "throttle_reasons": clocks.get("reasons"),
         **card(),
     }
+    if xent:
+        res["loss"] = "cross_entropy"
+        res["mse_model_ms_per_step"] = round(ms["mse_model"], 4)
+        res["step_overhead_vs_mse"] = round(ms["model"] / ms["mse_model"] - 1.0, 4)
+        res["xent_kernels"] = xent_kernel_times(ops, h, w2, b2, t, B, args.steps * args.reps)
     print(json.dumps(res), flush=True)
+
+
+def xent_kernel_times(ops, h, w2, b2, labels, B, calls):
+    """Device time per launch of gemm_bias_xent, xent_finish and gemm_bf16_tn on the output layer's shape, from a
+    torch.profiler run of its own (after the event-timed arms), and the bytes xent_finish moves."""
+    from torch.profiler import ProfilerActivity, profile
+
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(calls):
+            ops.linear_bias_xent_forward_local(h, w2, b2, labels, 1.0 / B, 1.0 / B)
+            ops.gemm_bf16_tn(h, w2)
+        torch.cuda.synchronize()
+    want = {"gemm_bias_xent": "gemm_bf16_wgmma_kernel<false, 5, false>", "xent_finish": "xent_finish_kernel",
+            "gemm_bf16_tn": "gemm_bf16_wgmma_kernel<false, 0, false>"}
+    times = {}
+    for ev in prof.key_averages():
+        for key, pattern in want.items():
+            if pattern in ev.key and ev.count >= calls:
+                times[key] = round(ev.device_time_total / ev.count / 1e3, 4)  # ms per launch
+    M, C = h.shape[0], w2.shape[0]
+    tiles = (C + 255) // 256
+    # logits read + dy written (bf16), column-sum partials written, tile pairs and labels read, row losses
+    moved = 2 * M * C * 2 + (M + 15) // 16 * C * 4 + tiles * M * 8 + M * 8 + 2 * M * 4
+    out = {"ms": times, "xent_finish_bytes": moved}
+    if "xent_finish" in times:
+        out["xent_finish_gb_per_s"] = round(moved / times["xent_finish"] / 1e6, 1)
+    if "gemm_bias_xent" in times and "gemm_bf16_tn" in times:
+        out["gemm_bias_xent_overhead"] = round(times["gemm_bias_xent"] / times["gemm_bf16_tn"] - 1.0, 4)
+    return out
 
 
 if __name__ == "__main__":

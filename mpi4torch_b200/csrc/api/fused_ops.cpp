@@ -348,6 +348,44 @@ std::tuple<Tensor, Tensor, Tensor> linear_bias_mse_forward_local(const Tensor& x
   return {dy, loss, part};
 }
 
+// Forward of the output layer with the softmax cross-entropy loss, against already averaged parameters:
+//   logits = bf16(x @ w^T + b),  lse[r] = log sum_c exp(logits[r, c]),
+//   dy = grad_scale * (softmax(logits) - onehot(labels))  (bf16, written over the logits),
+//   loss[1] = loss_scale * sum_r (lse[r] - logits[r, labels[r]]), summed in a fixed order,
+//   partials = fp32 column-sum partials of dy, as linear_bias_mse_forward_local returns them.
+// A row labelled ignore_index gets a zero dy row and adds nothing to the loss; any other label outside [0, C) makes
+// its dy row and the loss NaN (it is never used as an index).
+std::tuple<Tensor, Tensor, Tensor> linear_bias_xent_forward_local(const Tensor& x, const Tensor& w, const Tensor& b,
+                                                                  const Tensor& labels, double loss_scale,
+                                                                  double grad_scale, int64_t ignore_index) {
+  check_2d_bf16(x, "x");
+  check_2d_bf16(w, "w");
+  check_bias(b, w);
+  TORCH_CHECK(labels.is_cuda() && labels.device() == x.device() && labels.dim() == 1 &&
+                  labels.scalar_type() == at::kLong && labels.is_contiguous() && labels.size(0) == x.size(0),
+              "mpi4torch_b200: labels must be a contiguous 1-d int64 CUDA tensor with one label per row of x");
+  TORCH_CHECK(x.size(1) == w.size(1), "mpi4torch_b200: linear_bias_xent_forward_local shape mismatch");
+  TORCH_CHECK(x.size(0) > 0, "mpi4torch_b200: linear_bias_xent_forward_local needs a non-empty batch");
+  c10::cuda::CUDAGuard guard(x.device());
+  const int64_t M = x.size(0), C = w.size(0);
+  Tensor dy = at::empty({M, C}, x.options());
+  Tensor loss = at::empty({1}, x.options().dtype(at::kFloat));
+  Tensor part = colsum_workspace(M, C, x);
+  Tensor ms = at::empty({xent_tiles(C), M, 2}, x.options().dtype(at::kFloat));
+  Tensor row_loss = at::empty({M}, x.options().dtype(at::kFloat));
+  Tensor done = at::zeros({1}, x.options().dtype(at::kInt));
+  cudaStream_t stream = c10::cuda::getCurrentCUDAStream(x.device().index()).stream();
+  std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
+  float2* ms_ptr = reinterpret_cast<float2*>(ms.data_ptr<float>());
+  launch_gemm_bias_xent(x.data_ptr(), w.data_ptr(), b.data_ptr<float>(), dy.data_ptr(), ms_ptr, M, C, x.size(1),
+                        x.stride(0), w.stride(0), dy.stride(0), backend().device_comm().sm_count, stream);
+  launch_xent_finish(dy.data_ptr(), M, C, dy.stride(0), ms_ptr, labels.data_ptr<int64_t>(), ignore_index,
+                     static_cast<float>(loss_scale), static_cast<float>(grad_scale), row_loss.data_ptr<float>(),
+                     reinterpret_cast<unsigned int*>(done.data_ptr<int>()), loss.data_ptr<float>(), part.data_ptr<float>(),
+                     stream);
+  return {dy, loss, part};
+}
+
 // (dz, partials): dz = grad_scale * (dy @ w) * gelu_tanh'(z) in bf16 (w read in place as in gemm_bf16_nn), and the
 // fp32 column-sum partials of dz.
 std::tuple<Tensor, Tensor> gemm_nn_gelu_backward(const Tensor& dy, const Tensor& w, const Tensor& z,
@@ -389,6 +427,9 @@ TORCH_LIBRARY_FRAGMENT(mpi4torch_b200, m) {
   m.def("linear_bias_mse_forward_local(Tensor x, Tensor w, Tensor b, Tensor target, float loss_scale, float grad_scale) "
         "-> (Tensor, Tensor, Tensor)",
         &linear_bias_mse_forward_local);
+  m.def("linear_bias_xent_forward_local(Tensor x, Tensor w, Tensor b, Tensor labels, float loss_scale, float grad_scale, "
+        "int ignore_index=-100) -> (Tensor, Tensor, Tensor)",
+        &linear_bias_xent_forward_local);
   m.def("gemm_nn_gelu_backward(Tensor dy, Tensor w, Tensor z, Tensor? grad_scale=None) -> (Tensor, Tensor)",
         &gemm_nn_gelu_backward);
   m.def("column_sum(Tensor partials, Tensor? grad_scale=None) -> Tensor", &column_sum);

@@ -47,10 +47,11 @@ struct GemmArgs {
 // the fused kernel's communication warps need registers: half-width tiles there
 template <bool FUSED> constexpr int tile_n() { return FUSED ? 128 : 256; }
 
-// Epilogues of the two-layer MLP (EPI 2..4; unused by EPI 0/1):
+// Epilogues of the two-layer MLP (EPI 2..5; unused by EPI 0/1):
 //   EPI 2  TN  z = acc + bias -> C,  h = gelu_tanh(z) -> h_out
 //   EPI 3  TN  d = acc + bias - T:  C = grad_scale * d, loss as EPI 1, column-sum partials of C
 //   EPI 4  NN  C = gscale * acc * gelu_tanh'(z), z read from T (bf16), column-sum partials of C
+//   EPI 5  TN  C = logits = acc + bias, per-tile softmax partials (xent_epilogue; xent_finish completes them)
 // Column sums are deterministic: a warp adds its 16 rows in registers (h pair, then lane bits 2-4) and
 // lanes 0-3 store one fp32 row of colsum[ceil(M/16), N]; column_sum_kernel adds those rows in a fixed order.
 struct MlpEpiArgs {
@@ -58,6 +59,7 @@ struct MlpEpiArgs {
   void* h_out;          // EPI 2: bf16, same layout as C
   float* colsum;        // EPI 3, 4: [ceil(M/16), N] fp32, row-major
   const float* gscale;  // EPI 4: optional device scalar
+  float2* xent_ms;      // EPI 5: [ceil(N/256), M] (max, sum of exp) per row and column tile
 };
 
 constexpr float kGeluBeta = 0.7978845608028654f;  // sqrt(2/pi)
@@ -156,6 +158,63 @@ __device__ __forceinline__ void mlp_epilogue(const float (&acc)[BN / 2], const G
   }
 }
 
+// The one exponential of the cross-entropy path: the epilogue's tile sums and xent_finish's probabilities must use
+// the same function, or the softmax of a row would not add up to one.
+__device__ __forceinline__ float xent_exp(float v) { return expf(v); }
+
+// EPI 5  TN  logit = bf16(acc + bias) -> C, and for each row the pair (m, s) of this 256-column tile: m the max of
+// the row's stored (bf16-rounded) logits over the valid columns, s = sum exp(logit - m).  A thread reduces its 64
+// values of a row, the quad (lanes 4r .. 4r+3 hold one row) combines them, and its first lane stores the pair.
+// A -inf logit adds nothing to s without evaluating exp: a tile of -inf gives (-inf, 0), never exp(-inf - -inf).
+// NaN is dropped by fmaxf but reaches s through exp(NaN - m); +inf gives m = +inf and s = exp(inf - inf) = NaN.
+template <int BN>
+__device__ __forceinline__ void xent_epilogue(float (&acc)[BN / 2], const GemmArgs& g, const MlpEpiArgs& e, int m_blk,
+                                              int n_blk, int wgi) {
+  const int row0 = m_blk * BM + wgi * 64 + frag_row(0);
+  const bool row_ok[2] = {row0 < g.M, row0 + 8 < g.M};
+  float m[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int col = n_blk * BN + frag_col(j);
+    if (col >= g.N) continue;  // N is a multiple of 8: a column pair is wholly in or out
+    const float2 bv = *reinterpret_cast<const float2*>(e.bias + col);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint32_t p = pack_bf16x2(acc[4 * j + 2 * h] + bv.x, acc[4 * j + 2 * h + 1] + bv.y);
+      const float v0 = bf16_bits_to_float(static_cast<uint16_t>(p & 0xffffu));
+      const float v1 = bf16_bits_to_float(static_cast<uint16_t>(p >> 16));
+      acc[4 * j + 2 * h] = v0;
+      acc[4 * j + 2 * h + 1] = v1;
+      m[h] = fmaxf(m[h], fmaxf(v0, v1));
+      if (row_ok[h])
+        *reinterpret_cast<uint32_t*>(static_cast<uint16_t*>(g.C) + static_cast<int64_t>(row0 + 8 * h) * g.ldc + col) = p;
+    }
+  }
+  float s[2] = {0.f, 0.f};
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    m[h] = fmaxf(m[h], __shfl_xor_sync(0xffffffffu, m[h], 1));
+    m[h] = fmaxf(m[h], __shfl_xor_sync(0xffffffffu, m[h], 2));
+  }
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    if (n_blk * BN + frag_col(j) >= g.N) continue;
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const float v = acc[4 * j + 2 * h + i];
+        s[h] += v == -INFINITY ? 0.f : xent_exp(v - m[h]);
+      }
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    s[h] += __shfl_xor_sync(0xffffffffu, s[h], 1);
+    s[h] += __shfl_xor_sync(0xffffffffu, s[h], 2);
+    if ((threadIdx.x & 3) == 0 && row_ok[h]) e.xent_ms[static_cast<int64_t>(n_blk) * g.M + row0 + 8 * h] = make_float2(m[h], s[h]);
+  }
+}
+
 template <bool FUSED, int EPI, bool B_MN>
 __global__ void __launch_bounds__(kGemmThreads + (FUSED ? kCommWarps * 32 : 0), 1)
 gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
@@ -214,7 +273,9 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
       const int m_blk = t - n_blk * m_tiles;
       mma_tile<false, B_MN, BN>(acc, smem, pipe, stage, phase, k_blocks, wgi);
       float loss_part = 0.f;
-      if constexpr (EPI >= 2) {
+      if constexpr (EPI == 5) {
+        xent_epilogue<BN>(acc, g, e, m_blk, n_blk, wgi);
+      } else if constexpr (EPI >= 2) {
         mlp_epilogue<EPI, BN>(acc, g, e, m_blk, n_blk, wgi, loss_part);
       } else {
   #pragma unroll
@@ -321,6 +382,125 @@ __global__ void __launch_bounds__(256) column_sum_kernel(const float* __restrict
     for (int k = 1; k < 8; ++k) t += part[k][tx];
     out[n] = gscale != nullptr ? t * *gscale : t;
   }
+}
+
+constexpr int kXentRows = 16;  // rows per block: one row of the column-sum partials, as EPI 3 writes them
+constexpr int kXentThreads = 256;
+constexpr int kXentCols = 8 * kXentThreads;  // columns per block: 8 per thread, one 16-byte load per row
+
+// Completes EPI 5 in place over the logits y [M, N] (bf16, leading dimension ldy).  Block b covers rows
+// [16 r, 16 r + 16) and columns [2048 c, 2048 c + 2048) with r = b / col_blocks, c = b % col_blocks.
+//   1. lse of its 16 rows from the tile pairs ms[tile, row] = (m, s): M = max m, lse = M + log sum s exp(m - M).
+//      Thread (slot, row) visits tiles slot, slot + 16, ..; the 16 slots are then added in order.  A tile with
+//      s = 0 (all its logits -inf) is skipped, so exp(-inf - -inf) is never evaluated.
+//   2. dy = grad_scale (exp(logit - lse) - [col == label]) over the logits, and colsum[r, col] = sum of the 16 rows'
+//      fp32 dy in row order.  A row whose label is ignore_index gets dy = 0; one whose label is outside [0, N) NaN.
+//   3. The loss of row i is lse - logit[i, label] (0 if ignored, NaN if the label is out of range), stored in
+//      row_loss.  The last block to finish (an integer counter) adds row_loss in a fixed order: the same bits on
+//      every call, with no float atomics.
+__global__ void __launch_bounds__(kXentThreads) xent_finish_kernel(uint16_t* __restrict__ y, int64_t ldy,
+                                                                   const float2* __restrict__ ms, int tiles,
+                                                                   const int64_t* __restrict__ labels, int M, int N,
+                                                                   int64_t ignore_index, float loss_scale, float grad_scale,
+                                                                   float* __restrict__ row_loss, unsigned int* done,
+                                                                   float* __restrict__ loss, float* __restrict__ colsum) {
+  __shared__ float red[kXentThreads];
+  __shared__ float lse_s[kXentRows];
+  __shared__ int64_t lab_s[kXentRows];
+  __shared__ bool last;
+  const int t = threadIdx.x;
+  const int col_blocks = (N + kXentCols - 1) / kXentCols;
+  const int rg = static_cast<int>(blockIdx.x / col_blocks), cb = static_cast<int>(blockIdx.x % col_blocks);
+  const int r0 = rg * kXentRows;
+  {
+    const int row = t % kXentRows, slot = t / kXentRows, r = r0 + row;
+    constexpr int kSlots = kXentThreads / kXentRows;
+    float mx = -INFINITY;
+    if (r < M)
+      for (int j = slot; j < tiles; j += kSlots) mx = fmaxf(mx, ms[static_cast<int64_t>(j) * M + r].x);
+    red[t] = mx;
+    __syncthreads();
+    float big = -INFINITY;
+#pragma unroll
+    for (int k = 0; k < kSlots; ++k) big = fmaxf(big, red[k * kXentRows + row]);
+    __syncthreads();
+    float sum = 0.f;
+    if (r < M)
+      for (int j = slot; j < tiles; j += kSlots) {
+        const float2 p = ms[static_cast<int64_t>(j) * M + r];
+        if (p.y != 0.f) sum += p.y * xent_exp(p.x - big);
+      }
+    red[t] = sum;
+    __syncthreads();
+    if (slot == 0) {
+      float tot = 0.f;
+#pragma unroll
+      for (int k = 0; k < kSlots; ++k) tot += red[k * kXentRows + row];
+      lse_s[row] = big + logf(tot);
+      lab_s[row] = r < M ? labels[r] : ignore_index;
+    }
+    __syncthreads();
+  }
+  const int c = cb * kXentCols + 8 * t;
+  float cs[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  for (int i = 0; i < kXentRows && r0 + i < M; ++i) {
+    const int r = r0 + i;
+    const int64_t lab = lab_s[i];
+    const bool ignored = lab == ignore_index;
+    const bool valid = !ignored && lab >= 0 && lab < N;
+    // a label that is no column of the row: its loss is written once, by the first thread of column block 0
+    if (!valid && cb == 0 && t == 0) row_loss[r] = ignored ? 0.f : NAN;
+    if (c >= N) continue;
+    uint16_t* yr = y + static_cast<int64_t>(r) * ldy + c;
+    const uint4 raw = *reinterpret_cast<const uint4*>(yr);
+    const uint32_t w[4] = {raw.x, raw.y, raw.z, raw.w};
+    float v[8];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      v[2 * k] = bf16_bits_to_float(static_cast<uint16_t>(w[k] & 0xffffu));
+      v[2 * k + 1] = bf16_bits_to_float(static_cast<uint16_t>(w[k] >> 16));
+    }
+    const float lse = lse_s[i];
+    // In place: the store below overwrites logit[r, label], which the row's loss needs.  Only this thread holds
+    // that column, so it reads the logit here, from the registers loaded before its own store.
+    if (valid && lab >= c && lab < c + 8) {
+      float vl = 0.f;
+#pragma unroll
+      for (int k = 0; k < 8; ++k)
+        if (c + k == lab) vl = v[k];
+      row_loss[r] = lse - vl;
+    }
+    float d[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      d[k] = ignored ? 0.f : valid ? grad_scale * (xent_exp(v[k] - lse) - (c + k == lab ? 1.f : 0.f)) : NAN;
+      cs[k] += d[k];
+    }
+    *reinterpret_cast<uint4*>(yr) = make_uint4(pack_bf16x2(d[0], d[1]), pack_bf16x2(d[2], d[3]), pack_bf16x2(d[4], d[5]),
+                                               pack_bf16x2(d[6], d[7]));
+  }
+  if (c < N) {
+    float4* out = reinterpret_cast<float4*>(colsum + static_cast<int64_t>(rg) * N + c);
+    out[0] = make_float4(cs[0], cs[1], cs[2], cs[3]);
+    out[1] = make_float4(cs[4], cs[5], cs[6], cs[7]);
+  }
+  // every block's row losses are visible before its arrival on the counter
+  __threadfence();
+  __syncthreads();
+  if (t == 0) last = atomicAdd(done, 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  float part = 0.f;
+  for (int r = t; r < M; r += kXentThreads) part += __ldcg(row_loss + r);
+  red[t] = part;
+  __syncthreads();
+#pragma unroll
+  for (int s = kXentThreads / 2; s > 0; s >>= 1) {
+    if (t < s) red[t] += red[t + s];
+    __syncthreads();
+  }
+  if (t == 0) *loss = loss_scale * red[0];
 }
 
 GemmArgs plain_args(void* C, int64_t M, int64_t N, int64_t K, int64_t ldc) {
@@ -503,6 +683,36 @@ void launch_column_sum(const float* partial, int64_t rows, int64_t N, float* out
   cudaError_t err = cudaGetLastError();
   M4T_CHECK(err == cudaSuccess, "column_sum launch failed: " << cudaGetErrorString(err));
   note_kernel_launch("column_sum");
+}
+
+int64_t xent_tiles(int64_t N) { return (N + tile_n<false>() - 1) / tile_n<false>(); }
+
+void launch_gemm_bias_xent(const void* A, const void* B, const float* bias, void* logits, float2* ms, int64_t M,
+                           int64_t N, int64_t K, int64_t lda, int64_t ldb, int64_t ldc, int sm_count, cudaStream_t stream) {
+  M4T_CHECK(gemm_bf16_tn_supported(M, N, K, A, B, logits, lda, ldb, ldc),
+            "unsupported GEMM shape/alignment for the wgmma bias+cross-entropy path");
+  M4T_CHECK(epilogue_bias_ok(bias), "the bias needs an 8-byte-aligned base");
+  MlpEpiArgs e{};
+  e.bias = bias;
+  e.xent_ms = ms;
+  launch<false, 5, false>(plain_grid(M, N, sm_count), make_tmap(A, M, K, lda, BM), make_tmap(B, N, K, ldb, tile_n<false>()),
+                          plain_args(logits, M, N, K, ldc), CommArgs{}, stream, "gemm_bias_xent", e);
+}
+
+void launch_xent_finish(void* y, int64_t M, int64_t N, int64_t ldy, const float2* ms, const int64_t* labels,
+                        int64_t ignore_index, float loss_scale, float grad_scale, float* row_loss, unsigned int* done,
+                        float* loss, float* colsum, cudaStream_t stream) {
+  M4T_CHECK(M > 0 && N > 0 && N % 8 == 0 && ldy % 8 == 0 && ldy >= N && (reinterpret_cast<uintptr_t>(y) & 15u) == 0 &&
+                (reinterpret_cast<uintptr_t>(colsum) & 15u) == 0 && M < (1ll << 31) && N < (1ll << 31),
+            "xent_finish: unsupported shape or alignment");
+  const int64_t blocks = ((M + kXentRows - 1) / kXentRows) * ((N + kXentCols - 1) / kXentCols);
+  M4T_CHECK(blocks < (1ll << 31), "xent_finish: too many blocks");
+  xent_finish_kernel<<<static_cast<unsigned>(blocks), kXentThreads, 0, stream>>>(
+      static_cast<uint16_t*>(y), ldy, ms, static_cast<int>(xent_tiles(N)), labels, static_cast<int>(M), static_cast<int>(N),
+      ignore_index, loss_scale, grad_scale, row_loss, done, loss, colsum);
+  cudaError_t err = cudaGetLastError();
+  M4T_CHECK(err == cudaSuccess, "xent_finish launch failed: " << cudaGetErrorString(err));
+  note_kernel_launch("xent_finish");
 }
 
 int fused_gemm_grid(const DeviceComm& dc) { return std::min(dc.sm_count, kMaxChannels) & ~1; }

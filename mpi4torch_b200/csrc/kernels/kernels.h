@@ -148,6 +148,18 @@ void launch_gemm_nn_gelu_bwd_colsum(const void* A, const void* B, const void* z,
 // out[n] = gscale * sum_i partial[i, n], fp32, summed in a fixed order of i.
 void launch_column_sum(const float* partial, int64_t rows, int64_t N, float* out, const float* gscale,
                        cudaStream_t stream);
+// Softmax cross-entropy output layer, two kernels.  gemm_bias_xent: logits = bf16(A * B^T + bias) -> logits, and per
+// row and 256-column tile the pair (max, sum exp(logit - max)) of the stored logits -> ms [xent_tiles(N), M].
+int64_t xent_tiles(int64_t N);
+void launch_gemm_bias_xent(const void* A, const void* B, const float* bias, void* logits, float2* ms, int64_t M,
+                           int64_t N, int64_t K, int64_t lda, int64_t ldb, int64_t ldc, int sm_count, cudaStream_t stream);
+// xent_finish, in place over the logits: dy = grad_scale * (softmax - onehot(labels)) (bf16), colsum = partial
+// column sums of dy as launch_gemm_bias_mse_colsum writes them, *loss = loss_scale * sum_rows (lse - logit[label])
+// in a fixed order.  A label equal to ignore_index gives a zero row and loss 0, one outside [0, N) a NaN row and loss.
+// Workspaces: row_loss [M] fp32, done: one zeroed counter.
+void launch_xent_finish(void* y, int64_t M, int64_t N, int64_t ldy, const float2* ms, const int64_t* labels,
+                        int64_t ignore_index, float loss_scale, float grad_scale, float* row_loss, unsigned int* done,
+                        float* loss, float* colsum, cudaStream_t stream);
 
 // ---- weight gradient (wgrad_wgmma.cu) ------------------------------------------------
 // G[N,K] = dY[Mb,N]^T * X[Mb,K]: both operands MN-major, no transposed copies.

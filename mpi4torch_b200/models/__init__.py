@@ -4,6 +4,6 @@ examples/simple_linear_regression.py); BASELINE.json adds the 4096x4096
 data-parallel linear layer."""
 from .linear_regression import LinearRegression, make_regression_shard
 from .dp_linear import DPLinearModel
-from .dp_mlp import DPMLPModel
+from .dp_mlp import DPMLPClassifier, DPMLPModel
 
-__all__ = ["LinearRegression", "make_regression_shard", "DPLinearModel", "DPMLPModel"]
+__all__ = ["LinearRegression", "make_regression_shard", "DPLinearModel", "DPMLPModel", "DPMLPClassifier"]

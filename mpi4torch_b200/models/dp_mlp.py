@@ -11,13 +11,18 @@ One training step, every rank, on the autograd graph:
 With ``sgd_in_backward=False`` (or off the kernel path) the parameters get ordinary ``.grad`` tensors and
 ``train_step`` applies SGD.  Biases are fp32 when the weights are 16-bit: a bf16 bias would lose SGD updates
 below 2^-8 of its value.
+
+``DPMLPClassifier`` is the same model with a softmax cross-entropy loss over integer class labels
+(``dp_mlp_cross_entropy``); only the output layer's forward kernels differ.
 """
 from __future__ import annotations
 
 import torch
+import torch.nn.functional as F
 
 import mpi4torch_b200 as m4t
-from mpi4torch_b200.ops import InBackwardSGD, dp_mlp_mse, dp_mlp_mse_supported, mlp_in_backward_sgd_supported
+from mpi4torch_b200.ops import (InBackwardSGD, dp_mlp_cross_entropy, dp_mlp_cross_entropy_supported, dp_mlp_mse,
+                                dp_mlp_mse_supported, mlp_in_backward_sgd_supported)
 
 
 class DPMLPModel:
@@ -59,10 +64,13 @@ class DPMLPModel:
         key = (x.device, x.dtype, tuple(x.shape), tuple(x.stride()), tuple(target.shape))
         ok = self._opt_ok.get(key)
         if ok is None:
-            ok = (dp_mlp_mse_supported(x, self.w1, self.b1, self.w2, self.b2, target, self.comm)
+            ok = (self._kernels_supported(x, target)
                   and mlp_in_backward_sgd_supported(x, self.w1, self.w2, self.comm))
             self._opt_ok[key] = ok
         return ok
+
+    def _kernels_supported(self, x: torch.Tensor, target: torch.Tensor) -> bool:
+        return dp_mlp_mse_supported(x, self.w1, self.b1, self.w2, self.b2, target, self.comm)
 
     def loss(self, x: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
         """Global mean-squared-error loss as a differentiable one-element tensor."""
@@ -84,3 +92,43 @@ class DPMLPModel:
                         p.add_(p.grad, alpha=-self.lr)
                         p.grad = None
         return value.detach().reshape(())
+
+
+class DPMLPClassifier(DPMLPModel):
+    """The same MLP with ``num_classes`` outputs, trained with softmax cross-entropy (``dp_mlp_cross_entropy``).
+
+    ``loss(x, labels)`` is ``sum over every rank's non-ignored rows of CE / (B * P)``: rows labelled ``ignore_index``
+    add nothing to the numerator but still count in the denominator B * P, so with ignored rows this is not
+    ``F.cross_entropy``'s ``mean`` (which divides by the number of non-ignored rows).  ``train_step(x, labels)`` is
+    inherited.
+
+    The kernels need ``num_classes % 128 == 0``; other class counts run the torch composition.  To keep such a model
+    on the kernels, pad the classes: build it with ``num_classes`` rounded up to a multiple of 128 and set the padded
+    classes' bias to ``-inf`` (``model.b2.data[n:] = float("-inf")``).  Their logits are ``-inf``, so they get
+    probability 0 and gradient 0, their bias stays ``-inf``, and the loss and the real classes' gradients are those
+    of the unpadded model.  Read the first ``n`` columns of :meth:`logits`.
+    """
+
+    def __init__(self, in_features: int, hidden_features: int, num_classes: int, comm=None, device="cuda",
+                 dtype=torch.bfloat16, lr: float = 1e-4, seed: int = 0, sgd_in_backward: bool = True,
+                 prefetch: bool = True, ignore_index: int = -100):
+        super().__init__(in_features, hidden_features, num_classes, comm=comm, device=device, dtype=dtype, lr=lr,
+                         seed=seed, sgd_in_backward=sgd_in_backward, prefetch=prefetch)
+        self.ignore_index = ignore_index
+
+    def _kernels_supported(self, x: torch.Tensor, labels: torch.Tensor) -> bool:
+        return dp_mlp_cross_entropy_supported(x, self.w1, self.b1, self.w2, self.b2, labels, self.comm)
+
+    def loss(self, x: torch.Tensor, labels: torch.Tensor) -> torch.Tensor:
+        """Global cross-entropy loss (sum over non-ignored rows / (B * P)) as a differentiable one-element tensor."""
+        opts = self.optimizers if self._in_backward(x, labels) else None
+        local = dp_mlp_cross_entropy(x, self.w1, self.b1, self.w2, self.b2, labels, self.comm,
+                                     loss_scale=1.0 / (x.shape[0] * self.comm.size), ignore_index=self.ignore_index,
+                                     optimizers=opts)
+        return self.comm.Allreduce(local, m4t.MPI_SUM)
+
+    @torch.no_grad()
+    def logits(self, x: torch.Tensor) -> torch.Tensor:
+        """``h @ W2^T + b2`` with ``h = gelu_tanh(x @ W1^T + b1)``, this rank's parameters, for evaluation."""
+        h = F.gelu(F.linear(x, self.w1, self.b1.to(x.dtype)), approximate="tanh")
+        return F.linear(h, self.w2, self.b2.to(h.dtype))

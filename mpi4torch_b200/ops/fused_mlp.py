@@ -12,9 +12,14 @@ updated inside backward by the wgrad kernels (with P > 1: reduce-scatter -> SGD 
 the new weights for the next forward, one kernel per weight) and the biases by ``allreduce_axpy_``; the
 parameters then receive no ``.grad``.
 
+``dp_mlp_cross_entropy(x, W1, b1, W2, b2, labels, ...)``  loss_local = loss_scale * sum_rows CE(y, labels)
+    The same node with a softmax cross-entropy output layer: the second GEMM stores the bf16 logits and per-tile
+    softmax partials, and ``xent_finish`` turns the logits into dL/dy = loss_scale * (softmax(y) - onehot) in place,
+    with the loss and the same column-sum partials.  The backward is the MSE node's, unchanged.
+
 Elsewhere (CPU tensors, other dtypes, shapes the kernels reject, communicators created by ``Split``) the same
-math runs as the composition ``F.linear -> F.gelu(tanh) -> F.linear -> MSE`` on ``AllreduceFused`` averages,
-which gives the same gradients.
+math runs as the composition ``F.linear -> F.gelu(tanh) -> F.linear -> MSE`` (or ``F.cross_entropy``) on
+``AllreduceFused`` averages, which gives the same gradients.
 """
 from __future__ import annotations
 
@@ -44,24 +49,32 @@ def _update_weight(ops, comm, opt: InBackwardSGD, weight, dy, x, g) -> None:
         opt.remember(weight, None)
 
 
+def _mlp_forward(ctx, x, w1, b1, w2, b2, comm, opts, output_layer):
+    """Forward of the MLP nodes up to the loss: the parameter averages (or the prefetched ones), the bias + GELU GEMM,
+    then ``output_layer(ops, h, w2_avg, b2_avg) -> (dy, loss, dy_part)``, which stores dL/dy and its column-sum
+    partials.  Saves what :meth:`_DPMLPMSE.backward` reads."""
+    ops = _ops()
+    w1_avg = opts[0].take_prefetched(w1) if opts is not None else None
+    w2_avg = opts[1].take_prefetched(w2) if opts is not None else None
+    w1_avg = _average(comm, w1) if w1_avg is None else w1_avg
+    w2_avg = _average(comm, w2) if w2_avg is None else w2_avg
+    h, z = ops.linear_bias_gelu_forward(x, w1_avg, _average(comm, b1))
+    dy, local, dy_part = output_layer(ops, h, w2_avg, _average(comm, b2))
+    ctx.save_for_backward(x, h, z, dy, w1_avg, w2_avg, dy_part)
+    ctx.comm, ctx.opts, ctx.params = comm, opts, (w1, b1, w2, b2)
+    return local
+
+
 class _DPMLPMSE(torch.autograd.Function):
     """Local MSE loss of the data-parallel two-layer MLP; backward folds the upstream device scalar ``g``
     into the kernels' epilogues (never read on the host)."""
 
     @staticmethod
     def forward(ctx, x, w1, b1, w2, b2, target, comm_holder, loss_scale, opts):
-        comm = comm_holder[0]
-        ops = _ops()
-        w1_avg = opts[0].take_prefetched(w1) if opts is not None else None
-        w2_avg = opts[1].take_prefetched(w2) if opts is not None else None
-        w1_avg = _average(comm, w1) if w1_avg is None else w1_avg
-        w2_avg = _average(comm, w2) if w2_avg is None else w2_avg
-        h, z = ops.linear_bias_gelu_forward(x, w1_avg, _average(comm, b1))
-        dy, local, dy_part = ops.linear_bias_mse_forward_local(h, w2_avg, _average(comm, b2), target, loss_scale,
-                                                                2.0 * loss_scale)
-        ctx.save_for_backward(x, h, z, dy, w1_avg, w2_avg, dy_part)
-        ctx.comm, ctx.opts, ctx.params = comm, opts, (w1, b1, w2, b2)
-        return local
+        def output_layer(ops, h, w2_avg, b2_avg):
+            return ops.linear_bias_mse_forward_local(h, w2_avg, b2_avg, target, loss_scale, 2.0 * loss_scale)
+
+        return _mlp_forward(ctx, x, w1, b1, w2, b2, comm_holder[0], opts, output_layer)
 
     @staticmethod
     def backward(ctx, g):
@@ -104,8 +117,42 @@ class _DPMLPMSE(torch.autograd.Function):
         return gx, gw1, gb1, gw2, gb2, None, None, None, None
 
 
+class _DPMLPCrossEntropy(_DPMLPMSE):
+    """Local softmax cross-entropy loss of the data-parallel two-layer MLP.  Only the output layer differs from
+    :class:`_DPMLPMSE`: it stores ``dL/dy = loss_scale * (softmax(y) - onehot(labels))`` and its column-sum
+    partials, so the backward is inherited unchanged.  ``loss_args`` is ``(loss_scale, ignore_index)``."""
+
+    @staticmethod
+    def forward(ctx, x, w1, b1, w2, b2, labels, comm_holder, loss_args, opts):
+        loss_scale, ignore_index = loss_args
+
+        def output_layer(ops, h, w2_avg, b2_avg):
+            return ops.linear_bias_xent_forward_local(h, w2_avg, b2_avg, labels, loss_scale, loss_scale, ignore_index)
+
+        return _mlp_forward(ctx, x, w1, b1, w2, b2, comm_holder[0], opts, output_layer)
+
+
 def _kernel_ops_present() -> bool:
     return hasattr(_ops(), "linear_bias_gelu_forward")
+
+
+def _mlp_kernels_supported(x, w1, b1, w2, b2, c) -> bool:
+    """The rules both MLP losses share: D, H, O multiples of 128, the batch a multiple of 64, contiguous bf16 weights
+    and input, contiguous fp32 biases, every operand of the two forward GEMMs aligned as the kernels read it."""
+    if not (c.is_world and m4t.cuda_backend_ready() and _kernel_ops_present()):
+        return False
+    if not all(t.is_cuda and t.dim() == 2 and t.dtype == torch.bfloat16 and t.is_contiguous() for t in (x, w1, w2)):
+        return False
+    if not all(b.is_cuda and b.dim() == 1 and b.dtype == torch.float32 and b.is_contiguous() for b in (b1, b2)):
+        return False
+    (B, D), (H, D1), (O, H1) = x.shape, w1.shape, w2.shape
+    if not (D1 == D and H1 == H and b1.shape[0] == H and b2.shape[0] == O):
+        return False
+    if not (B % 64 == 0 and D % 128 == 0 and H % 128 == 0 and O % 128 == 0 and B > 0):
+        return False
+    # base alignment and row strides of every operand the two forward GEMMs read (h is allocated by the first)
+    ops = _ops()
+    return bool(ops.gemm_bf16_tn_supported(x, w1, None, b1) and ops.gemm_bf16_tn_supported(x.new_empty((B, H)), w2, None, b2))
 
 
 def dp_mlp_mse_supported(x: torch.Tensor, w1: torch.Tensor, b1: torch.Tensor, w2: torch.Tensor, b2: torch.Tensor,
@@ -114,22 +161,24 @@ def dp_mlp_mse_supported(x: torch.Tensor, w1: torch.Tensor, b1: torch.Tensor, w2
     D, H, O must be multiples of 128, the batch a multiple of 64, and every operand aligned as the kernels read
     it (see ``gemm_bf16_tn_supported``)."""
     c = m4t.COMM_WORLD if comm is None else comm
-    if not (c.is_world and m4t.cuda_backend_ready() and _kernel_ops_present()):
+    if not _mlp_kernels_supported(x, w1, b1, w2, b2, c):
         return False
-    ts = (x, w1, w2, target)
-    if not all(t.is_cuda and t.dim() == 2 and t.dtype == torch.bfloat16 and t.is_contiguous() for t in ts):
+    if not (target.is_cuda and target.dim() == 2 and target.dtype == torch.bfloat16 and target.is_contiguous()
+            and tuple(target.shape) == (x.shape[0], w2.shape[0])):
         return False
-    if not all(b.is_cuda and b.dim() == 1 and b.dtype == torch.float32 and b.is_contiguous() for b in (b1, b2)):
+    return bool(_ops().gemm_bf16_tn_supported(x.new_empty((x.shape[0], w1.shape[0])), w2, target, b2))
+
+
+def dp_mlp_cross_entropy_supported(x: torch.Tensor, w1: torch.Tensor, b1: torch.Tensor, w2: torch.Tensor,
+                                   b2: torch.Tensor, labels: torch.Tensor, comm=None) -> bool:
+    """Does :func:`dp_mlp_cross_entropy` run on the library's kernels for these tensors (plain-gradient mode)?
+    The rules of :func:`dp_mlp_mse_supported` (C = number of classes in place of O), and ``labels`` a contiguous
+    1-d int64 CUDA tensor with one label per row."""
+    c = m4t.COMM_WORLD if comm is None else comm
+    if not (labels.is_cuda and labels.dim() == 1 and labels.dtype == torch.int64 and labels.is_contiguous()
+            and x.dim() == 2 and labels.shape[0] == x.shape[0] and labels.device == x.device):
         return False
-    (B, D), (H, D1), (O, H1) = x.shape, w1.shape, w2.shape
-    if not (D1 == D and H1 == H and b1.shape[0] == H and b2.shape[0] == O and tuple(target.shape) == (B, O)):
-        return False
-    if not (B % 64 == 0 and D % 128 == 0 and H % 128 == 0 and O % 128 == 0 and B > 0):
-        return False
-    # base alignment and row strides of every operand the two forward GEMMs read (h is allocated by the first)
-    ops = _ops()
-    return bool(ops.gemm_bf16_tn_supported(x, w1, None, b1)
-                and ops.gemm_bf16_tn_supported(x.new_empty((B, H)), w2, target, b2))
+    return _mlp_kernels_supported(x, w1, b1, w2, b2, c) and hasattr(_ops(), "linear_bias_xent_forward_local")
 
 
 def mlp_in_backward_sgd_supported(x: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, comm=None) -> bool:
@@ -156,18 +205,53 @@ def dp_mlp_mse(x: torch.Tensor, w1: torch.Tensor, b1: torch.Tensor, w2: torch.Te
     step to ``(w1, b1)`` and ``(w2, b2)`` itself; the parameters then receive no ``.grad``."""
     c = m4t.COMM_WORLD if comm is None else comm
     if dp_mlp_mse_supported(x, w1, b1, w2, b2, target, c):
-        if optimizers is not None:
-            if len(optimizers) != 2:
-                raise ValueError("mpi4torch_b200: dp_mlp_mse takes one InBackwardSGD per layer")
-            if not mlp_in_backward_sgd_supported(x, w1, w2, c):
-                raise RuntimeError("mpi4torch_b200: InBackwardSGD for the MLP needs, with more than one rank, bf16 weights "
-                                   "from symmetric_empty() with D, H, O % 256 == 0 and batch % 128 == 0")
-            optimizers = tuple(optimizers)
+        optimizers = _kernel_optimizers("dp_mlp_mse", optimizers, x, w1, w2, c)
         return _DPMLPMSE.apply(x, w1, b1, w2, b2, target, [c], float(loss_scale), optimizers)
+    y, acc = _composition(x, w1, b1, w2, b2, c, optimizers)
+    return ((y.to(acc) - target.to(acc)).square().sum() * loss_scale).reshape(1)
+
+
+def dp_mlp_cross_entropy(x: torch.Tensor, w1: torch.Tensor, b1: torch.Tensor, w2: torch.Tensor, b2: torch.Tensor,
+                         labels: torch.Tensor, comm=None, *, loss_scale: float, ignore_index: int = -100,
+                         optimizers: Optional[Sequence[InBackwardSGD]] = None) -> torch.Tensor:
+    """``loss_scale * sum_rows cross_entropy(MLP(x), labels)`` of THIS rank's batch (``F.cross_entropy`` with
+    ``reduction="sum"``) as a differentiable one-element fp32 tensor, with every parameter averaged over ranks;
+    sum it over ranks with ``comm.Allreduce``.  ``labels``: one int64 class index per row of ``x``.  A row labelled
+    ``ignore_index`` adds nothing to the loss or the gradients.  On the kernel path any other label outside
+    ``[0, C)`` makes the loss NaN (``F.cross_entropy`` raises instead).
+
+    The softmax is taken over the bf16 logits ``bf16(h @ W2^T + b2)``.  ``optimizers`` as in :func:`dp_mlp_mse`.
+    The kernels need C % 128 == 0: pad the classes to the next multiple of 128 and give the padded classes bias
+    ``-inf``, which gives them probability 0 and gradient 0, so their bias stays ``-inf``."""
+    if not (labels.dim() == 1 and labels.dtype == torch.int64 and x.dim() == 2 and labels.shape[0] == x.shape[0]):
+        raise ValueError(f"mpi4torch_b200: dp_mlp_cross_entropy needs int64 labels of shape ({x.shape[0]},), got "
+                         f"{labels.dtype} of shape {tuple(labels.shape)}")
+    c = m4t.COMM_WORLD if comm is None else comm
+    if dp_mlp_cross_entropy_supported(x, w1, b1, w2, b2, labels, c):
+        optimizers = _kernel_optimizers("dp_mlp_cross_entropy", optimizers, x, w1, w2, c)
+        return _DPMLPCrossEntropy.apply(x, w1, b1, w2, b2, labels, [c], (float(loss_scale), int(ignore_index)),
+                                        optimizers)
+    y, acc = _composition(x, w1, b1, w2, b2, c, optimizers)
+    return (F.cross_entropy(y.to(acc), labels, reduction="sum", ignore_index=ignore_index) * loss_scale).reshape(1)
+
+
+def _kernel_optimizers(name, optimizers, x, w1, w2, c):
+    if optimizers is None:
+        return None
+    if len(optimizers) != 2:
+        raise ValueError(f"mpi4torch_b200: {name} takes one InBackwardSGD per layer")
+    if not mlp_in_backward_sgd_supported(x, w1, w2, c):
+        raise RuntimeError("mpi4torch_b200: InBackwardSGD for the MLP needs, with more than one rank, bf16 weights "
+                           "from symmetric_empty() with D, H, O % 256 == 0 and batch % 128 == 0")
+    return tuple(optimizers)
+
+
+def _composition(x, w1, b1, w2, b2, c, optimizers):
+    """Off the kernel path: the MLP output ``y`` as the torch composition on ``AllreduceFused`` averages, and the
+    dtype the loss accumulates in (fp32; fp64 inputs stay fp64)."""
     if optimizers is not None:
         raise RuntimeError("mpi4torch_b200: InBackwardSGD is only available on the CUDA kernel path")
     avg = lambda p: c.AllreduceFused(p, m4t.MPI_SUM, 1.0 / c.size, None)  # noqa: E731
-    acc = torch.float64 if x.dtype == torch.float64 else torch.float32  # accumulate in fp32 (fp64 inputs stay fp64)
+    acc = torch.float64 if x.dtype == torch.float64 else torch.float32
     h = F.gelu(F.linear(x, avg(w1), avg(b1).to(x.dtype)), approximate="tanh")
-    y = F.linear(h, avg(w2), avg(b2).to(h.dtype))
-    return ((y.to(acc) - target.to(acc)).square().sum() * loss_scale).reshape(1)
+    return F.linear(h, avg(w2), avg(b2).to(h.dtype)), acc
