@@ -22,8 +22,17 @@ inline CUresult encode_tiled_2d(CUtensorMap* map, CUtensorMapDataType dt, void* 
     return reinterpret_cast<Fn>(p);
   }();
   const cuuint32_t estr[2] = {1, 1};
-  return fn(map, dt, 2, base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
-            CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = fn(map, dt, 2, base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
+                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r == CUDA_ERROR_INVALID_CONTEXT) {
+    // A thread that has made no runtime call yet, such as autograd's CUDA worker thread running a node's backward,
+    // has no current context; cudaFree(nullptr) binds the device's primary context to it.
+    const cudaError_t e = cudaFree(nullptr);
+    M4T_CHECK(e == cudaSuccess, "cudaFree(nullptr) failed: " << cudaGetErrorString(e));
+    r = fn(map, dt, 2, base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
+           CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  }
+  return r;
 }
 
 // Row-major [rows, cols] bf16 matrix with leading dimension `ld` (elements); boxes of

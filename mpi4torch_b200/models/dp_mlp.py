@@ -9,7 +9,10 @@ One training step, every rank, on the autograd graph:
                                                weight average inside them), column sums -> bias updates
 
 With ``sgd_in_backward=False`` (or off the kernel path) the parameters get ordinary ``.grad`` tensors and
-``train_step`` applies SGD.  Biases are fp32 when the weights are 16-bit: a bf16 bias would lose SGD updates
+``train_step`` applies SGD.  With ``sgd_in_backward=True`` a parameter set to ``requires_grad_(False)`` is not
+updated, and each ``loss()`` needs its ``backward()`` before the next ``loss()`` is computed: a backward whose
+forward came before another backward's weight update raises ``RuntimeError``, because its saved weights were
+overwritten.  So summing two losses and calling ``backward()`` once raises, after applying one of the two updates.  Biases are fp32 when the weights are 16-bit: a bf16 bias would lose SGD updates
 below 2^-8 of its value.
 
 ``DPMLPClassifier`` is the same model with a softmax cross-entropy loss over integer class labels

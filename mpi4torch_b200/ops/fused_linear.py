@@ -43,6 +43,10 @@ class InBackwardSGD:
     kernel has already all-reduced the NEW weights (x 1/size) into a symmetric buffer, so the next
     forward is a plain local GEMM.  The prefetch is dropped whenever the weight's version counter
     shows a modification the kernel did not make.
+
+    ``updates`` counts the in-place weight updates applied through this optimizer.  The kernels write
+    the weight through its data pointer, which torch's version counter does not see, so a node that
+    saved the weight (or its prefetched average) for backward compares this count instead.
     """
 
     def __init__(self, lr: float, prefetch: bool = True, assume_replicated: bool = False):
@@ -56,6 +60,7 @@ class InBackwardSGD:
         self._wavg: Optional[torch.Tensor] = None
         self._weight_id = None
         self._version = -1
+        self.updates = 0
 
     def take_prefetched(self, weight: torch.Tensor) -> Optional[torch.Tensor]:
         w_avg, self._wavg = self._wavg, None
@@ -167,6 +172,7 @@ class _DPLinearMSE(torch.autograd.Function):
             if opt is not None:
                 # optimizer-in-backward: the weight is updated by the kernel, no .grad is produced
                 scale = -opt.lr / comm.size
+                opt.updates += 1
                 if comm.size == 1:
                     ops.wgrad_sgd_(weight, dy, x, scale, g)
                     opt.remember(weight, None)

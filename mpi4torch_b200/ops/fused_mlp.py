@@ -39,6 +39,7 @@ def _average(comm, p: torch.Tensor) -> torch.Tensor:
 
 def _update_weight(ops, comm, opt: InBackwardSGD, weight, dy, x, g) -> None:
     scale = -opt.lr / comm.size
+    opt.updates += 1
     if comm.size == 1:
         ops.wgrad_sgd_(weight, dy, x, scale, g)
         opt.remember(weight, None)
@@ -62,6 +63,9 @@ def _mlp_forward(ctx, x, w1, b1, w2, b2, comm, opts, output_layer):
     dy, local, dy_part = output_layer(ops, h, w2_avg, _average(comm, b2))
     ctx.save_for_backward(x, h, z, dy, w1_avg, w2_avg, dy_part)
     ctx.comm, ctx.opts, ctx.params = comm, opts, (w1, b1, w2, b2)
+    # w1_avg / w2_avg are the weights themselves (P = 1) or the prefetch buffers (P > 1), which the next in-backward
+    # update rewrites without bumping torch's version counter: backward checks these counts instead
+    ctx.opt_updates = None if opts is None else (opts[0].updates, opts[1].updates)
     return local
 
 
@@ -81,6 +85,10 @@ class _DPMLPMSE(torch.autograd.Function):
         x, h, z, dy, w1_avg, w2_avg, dy_part = ctx.saved_tensors
         comm, opts = ctx.comm, ctx.opts
         w1, b1, w2, b2 = ctx.params
+        if opts is not None and (opts[0].updates, opts[1].updates) != ctx.opt_updates:
+            raise RuntimeError("mpi4torch_b200: the MLP weights were updated in place by another backward since this "
+                               "node's forward, so its saved weights are stale; with InBackwardSGD, run one backward "
+                               "per forward")
         ops = _ops()
         g = g.reshape(1).to(torch.float32)
         need = ctx.needs_input_grad
@@ -91,24 +99,29 @@ class _DPMLPMSE(torch.autograd.Function):
         # into a peer's buffer only after every rank's partial gradients of that tile have arrived, and a rank
         # produces its partials only after its own earlier reads, which come first in its stream.
         #   1. dz reads W2_avg;  2. layer-2 update;  3. dx reads W1_avg;  4. layer-1 update;  5. biases.
+        # In-backward mode updates only the parameters that require a gradient, so a frozen one stays as it is.
         dz, dz_part = ops.gemm_nn_gelu_backward(dy, w2_avg, z, g)
         gx = gw1 = gb1 = gw2 = gb2 = None
         if opts is not None:
-            _update_weight(ops, comm, opts[1], w2, dy, h, g)
+            if need[3]:
+                _update_weight(ops, comm, opts[1], w2, dy, h, g)
         elif need[3]:
             gw2 = comm.AllreduceFused(ops.wgrad_bf16(dy, h, g), m4t.MPI_SUM, 1.0 / comm.size, None)
         if need[0]:
             gx = ops.gemm_bf16_nn(dz, w1_avg)
         if opts is not None:
-            _update_weight(ops, comm, opts[0], w1, dz, x, None)
+            if need[1]:
+                _update_weight(ops, comm, opts[0], w1, dz, x, None)
         elif need[1]:
             gw1 = comm.AllreduceFused(ops.wgrad_bf16(dz, x, None), m4t.MPI_SUM, 1.0 / comm.size, None)
         db2 = ops.column_sum(dy_part, g)
         db1 = ops.column_sum(dz_part, None)
         if opts is not None:
             # one path for every P, summed in a fixed order: the biases stay bit-identical across ranks
-            ops.allreduce_axpy_(b2, db2, -opts[1].lr / comm.size)
-            ops.allreduce_axpy_(b1, db1, -opts[0].lr / comm.size)
+            if need[4]:
+                ops.allreduce_axpy_(b2, db2, -opts[1].lr / comm.size)
+            if need[2]:
+                ops.allreduce_axpy_(b1, db1, -opts[0].lr / comm.size)
         else:
             if need[4]:
                 gb2 = comm.AllreduceFused(db2, m4t.MPI_SUM, 1.0 / comm.size, None)
@@ -202,7 +215,13 @@ def dp_mlp_mse(x: torch.Tensor, w1: torch.Tensor, b1: torch.Tensor, w2: torch.Te
     tensor, with every parameter averaged over ranks; sum it over ranks with ``comm.Allreduce``.
 
     ``optimizers``: ``(opt1, opt2)``, one :class:`InBackwardSGD` per layer, makes ``backward`` apply the SGD
-    step to ``(w1, b1)`` and ``(w2, b2)`` itself; the parameters then receive no ``.grad``."""
+    step to ``(w1, b1)`` and ``(w2, b2)`` itself; the parameters then receive no ``.grad``.  Two rules hold in
+    that mode:
+      * only parameters with ``requires_grad`` are updated: a frozen weight or bias stays unchanged;
+      * run one backward per forward.  Backward reads the weights (or their prefetched averages) as they were at
+        this node's forward, and another node's backward updates them in place, so a node whose weights were
+        updated since its forward raises ``RuntimeError`` instead of computing its gradients from the new ones.
+        For example ``(model.loss(xa, ta) + model.loss(xb, tb)).backward()`` raises after applying one update."""
     c = m4t.COMM_WORLD if comm is None else comm
     if dp_mlp_mse_supported(x, w1, b1, w2, b2, target, c):
         optimizers = _kernel_optimizers("dp_mlp_mse", optimizers, x, w1, w2, c)
@@ -220,7 +239,8 @@ def dp_mlp_cross_entropy(x: torch.Tensor, w1: torch.Tensor, b1: torch.Tensor, w2
     ``ignore_index`` adds nothing to the loss or the gradients.  On the kernel path any other label outside
     ``[0, C)`` makes the loss NaN (``F.cross_entropy`` raises instead).
 
-    The softmax is taken over the bf16 logits ``bf16(h @ W2^T + b2)``.  ``optimizers`` as in :func:`dp_mlp_mse`.
+    The softmax is taken over the bf16 logits ``bf16(h @ W2^T + b2)``.  ``optimizers`` as in :func:`dp_mlp_mse`,
+    with the same two rules: frozen parameters are not updated, and one backward per forward.
     The kernels need C % 128 == 0: pad the classes to the next multiple of 128 and give the padded classes bias
     ``-inf``, which gives them probability 0 and gradient 0, so their bias stays ``-inf``."""
     if not (labels.dim() == 1 and labels.dtype == torch.int64 and x.dim() == 2 and labels.shape[0] == x.shape[0]):

@@ -77,19 +77,19 @@ WGRAD_EDGE_SHAPES = [(64, 128, 128), (64, 256, 896), (128, 384, 256), (192, 128,
 # ------------------------------------------------------------------------------------------------------------------
 # Exact inputs
 # ------------------------------------------------------------------------------------------------------------------
-def _gen(*vals):
-    return torch.Generator(device="cuda").manual_seed(sum((i + 1) * 7919 * int(v) for i, v in enumerate(vals)) % (2 ** 62))
+def _gen(*vals, device="cuda"):
+    return torch.Generator(device=device).manual_seed(sum((i + 1) * 7919 * int(v) for i, v in enumerate(vals)) % (2 ** 62))
 
 
 def ints(shape, r, gen, scale=1.0):
-    """float64 integers uniform in [-r, r], times `scale` (a power of two)."""
-    return torch.randint(-r, r + 1, shape, generator=gen, device="cuda", dtype=torch.int64).double() * scale
+    """float64 integers uniform in [-r, r], times `scale` (a power of two), on the generator's device."""
+    return torch.randint(-r, r + 1, shape, generator=gen, device=gen.device, dtype=torch.int64).double() * scale
 
 
 def ternary(shape, density, gen, scale=1.0):
-    """float64 values in {-1, 0, 1} (nonzero with probability `density`), times `scale`."""
-    sign = torch.randint(0, 2, shape, generator=gen, device="cuda", dtype=torch.int64).double() * 2 - 1
-    keep = torch.rand(shape, generator=gen, device="cuda", dtype=torch.float64) < density
+    """float64 values in {-1, 0, 1} (nonzero with probability `density`), times `scale`, on the generator's device."""
+    sign = torch.randint(0, 2, shape, generator=gen, device=gen.device, dtype=torch.int64).double() * 2 - 1
+    keep = torch.rand(shape, generator=gen, device=gen.device, dtype=torch.float64) < density
     return sign * keep * scale
 
 
