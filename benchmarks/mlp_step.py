@@ -9,6 +9,11 @@ with device events.  Prints one JSON line.
 ``--loss cross_entropy`` times DPMLPClassifier (softmax cross-entropy over O classes) against the eager composition
 with ``F.cross_entropy``, ``gemm_bias_xent`` against ``gemm_bf16_tn``, and ``xent_finish`` alone (as the whole
 cross-entropy op minus its GEMM), with the bytes xent_finish moves.
+
+``--micro-batches K [K ...]`` (MSE) adds gradient accumulation: the DPMLPModel step with ``train_step(x, t,
+micro_batches=K)`` for each K, alternated with the K = 1 in-backward step, the eager composition with K
+``backward()`` calls into ``.grad`` and then SGD, and, from a torch.profiler run of its own, ``wgrad_accumulate_``
+against ``wgrad_bf16`` and ``wgrad_sgd_`` on the first layer's micro-batch shape, next to the bytes each moves.
 """
 import argparse
 import json
@@ -58,7 +63,11 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--reps", type=int, default=3, help="alternations of the arms; medians are reported")
     ap.add_argument("--loss", choices=("mse", "cross_entropy"), default="mse")
+    ap.add_argument("--micro-batches", type=int, nargs="+", default=[],
+                    help="gradient-accumulation arms: micro-batches per step (each must divide --batch)")
     args = ap.parse_args()
+    if args.micro_batches and args.loss != "mse":
+        raise SystemExit("--micro-batches times the MSE model")
     if not torch.cuda.is_available():
         raise SystemExit("mlp_step.py needs a GPU")
     comm = m4t.COMM_WORLD
@@ -84,10 +93,11 @@ def main():
     lin2 = torch.nn.Linear(H, O, device="cuda", dtype=torch.bfloat16)
     eager_params = list(lin1.parameters()) + list(lin2.parameters())
 
-    def eager_step():
-        y = lin2(F.gelu(lin1(x), approximate="tanh"))
-        loss = F.cross_entropy(y.float(), t) if xent else (y.float() - t.float()).square().mean()
-        loss.backward()
+    def eager_step(K=1):
+        for xc, tc in zip(x.split(B // K), t.split(B // K)):  # K backward() calls add into .grad
+            y = lin2(F.gelu(lin1(xc), approximate="tanh"))
+            loss = F.cross_entropy(y.float(), tc) if xent else (y.float() - tc.float()).square().mean()
+            (loss if K == 1 else loss / K).backward()
         with torch.no_grad():
             grads = [p.grad for p in eager_params]
             torch._foreach_add_(eager_params, grads, alpha=-lr)
@@ -117,6 +127,9 @@ def main():
     for name, (new, plain) in pairs.items():
         arms[name] = new
         arms[name + ":plain"] = plain
+    for K in args.micro_batches:
+        arms[f"model_k{K}"] = lambda K=K: model.train_step(x, t, micro_batches=K)
+        arms[f"eager_k{K}"] = lambda K=K: eager_step(K)
     if xent:  # the MSE step of the same shape, alternated with the others
         mse_model = DPMLPModel(D, H, O, comm, device="cuda", lr=lr, seed=0)
         t_mse = torch.randn(B, O, device="cuda", generator=g).to(torch.bfloat16)
@@ -154,12 +167,51 @@ def main():
         "throttle_reasons": clocks.get("reasons"),
         **card(),
     }
+    if args.micro_batches:
+        res["micro_batches"] = {
+            K: {"model_ms_per_step": round(ms[f"model_k{K}"], 4), "eager_ms_per_step": round(ms[f"eager_k{K}"], 4),
+                "vs_k1_in_backward": round(ms[f"model_k{K}"] / ms["model"] - 1.0, 4)} for K in args.micro_batches}
+        Bc = B // max(args.micro_batches)
+        dz = torch.randn(Bc, H, device="cuda", generator=g).to(torch.bfloat16)
+        res["wgrad_kernels"] = wgrad_kernel_times(ops, dz, x[:Bc], args.steps * args.reps)
     if xent:
         res["loss"] = "cross_entropy"
         res["mse_model_ms_per_step"] = round(ms["mse_model"], 4)
         res["step_overhead_vs_mse"] = round(ms["model"] / ms["mse_model"] - 1.0, 4)
         res["xent_kernels"] = xent_kernel_times(ops, h, w2, b2, t, B, args.steps * args.reps)
     print(json.dumps(res), flush=True)
+
+
+def wgrad_kernel_times(ops, dy, x, calls):
+    """Device time per launch of wgrad_accumulate_, wgrad_bf16 and wgrad_sgd_ for G [N, K] = dy[Mb, N]^T x[Mb, K], each
+    in a torch.profiler run of its own (the plain and SGD ops are one kernel instantiation), and the bytes each
+    epilogue moves: 8 N K for the fp32 read-modify-write, 2 N K for the bf16 store, 4 N K for the SGD's bf16
+    read-modify-write."""
+    from torch.profiler import ProfilerActivity, profile
+
+    N, K = dy.shape[1], x.shape[1]
+    acc = torch.zeros(N, K, device="cuda")
+    w = torch.zeros(N, K, device="cuda", dtype=torch.bfloat16)
+    gs = torch.ones(1, device="cuda")
+    runs = {"wgrad_accumulate": (lambda: ops.wgrad_accumulate_(acc, dy, x, gs), 8),
+            "wgrad_bf16": (lambda: ops.wgrad_bf16(dy, x, gs), 2),
+            "wgrad_sgd": (lambda: ops.wgrad_sgd_(w, dy, x, -1e-30, gs), 4)}
+    out = {"shape": {"Mb": dy.shape[0], "N": N, "K": K}}
+    for name, (fn, bytes_per_elem) in runs.items():
+        fn()
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(calls):
+                fn()
+            torch.cuda.synchronize()
+        ev = [e for e in prof.key_averages() if "wgrad_bf16_wgmma_kernel" in e.key and e.count >= calls]
+        moved = bytes_per_elem * N * K
+        entry = {"epilogue_bytes": moved}
+        if len(ev) == 1:
+            t_ms = ev[0].device_time_total / ev[0].count / 1e3
+            entry.update(ms=round(t_ms, 4), epilogue_gb_per_s=round(moved / t_ms / 1e6, 1))
+        out[name] = entry
+    return out
 
 
 def xent_kernel_times(ops, h, w2, b2, labels, B, calls):

@@ -229,6 +229,30 @@ bool wgrad_bf16_ok(const Tensor& dy, const Tensor& x) {
                               x.stride(0), x.size(1));
 }
 
+// The rules of wgrad_bf16_supported, and acc a contiguous, 16-byte-aligned fp32 [N, K] tensor on x's device.
+bool wgrad_accumulate_ok(const Tensor& acc, const Tensor& dy, const Tensor& x) {
+  if (!wgrad_bf16_ok(dy, x)) return false;
+  if (!(acc.is_cuda() && acc.device() == x.device() && dy.device() == x.device() && acc.dim() == 2 &&
+        acc.scalar_type() == at::kFloat && acc.is_contiguous() && acc.size(0) == dy.size(1) && acc.size(1) == x.size(1)))
+    return false;
+  return wgrad_accumulate_supported(dy.size(0), dy.size(1), x.size(1), dy.data_ptr(), x.data_ptr(), acc.data_ptr<float>(),
+                                    dy.stride(0), x.stride(0));
+}
+
+// acc += grad_scale * dy^T @ x, accumulated in fp32 by the wgrad kernel's epilogue with one fmaf per element
+// (gradient accumulation over micro-batches).  Not a collective.
+void wgrad_accumulate_(Tensor acc, const Tensor& dy, const Tensor& x, const c10::optional<Tensor>& grad_scale) {
+  TORCH_CHECK(wgrad_accumulate_ok(acc, dy, x),
+              "mpi4torch_b200: wgrad_accumulate_ needs bf16 dy [B, N] and x [B, K] with unit inner strides, N % 128 == "
+              "K % 128 == B % 64 == 0, 16-byte-aligned operands, and acc a contiguous 16-byte-aligned fp32 [N, K] "
+              "tensor on the same device");
+  c10::cuda::CUDAGuard guard(x.device());
+  std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
+  launch_wgrad_accumulate(dy.data_ptr(), x.data_ptr(), acc.data_ptr<float>(), dy.size(0), dy.size(1), x.size(1),
+                          dy.stride(0), x.stride(0), backend().device_comm().sm_count,
+                          c10::cuda::getCurrentCUDAStream(x.device().index()).stream(), grad_scale_ptr(grad_scale, x));
+}
+
 bool wgrad_allreduce_sgd_supported(const Tensor& w, const Tensor& dy, const Tensor& x) {
   if (!World::instance().cuda_ready() || !wgrad_bf16_ok(dy, x)) return false;
   if (!(w.is_cuda() && w.dim() == 2 && w.scalar_type() == at::kBFloat16 && w.is_contiguous() &&
@@ -440,6 +464,8 @@ TORCH_LIBRARY_FRAGMENT(mpi4torch_b200, m) {
         &linear_mse_forward_local);
   m.def("wgrad_bf16(Tensor dy, Tensor x, Tensor? grad_scale=None) -> Tensor", &wgrad_bf16);
   m.def("wgrad_bf16_supported(Tensor dy, Tensor x) -> bool", &wgrad_bf16_ok);
+  m.def("wgrad_accumulate_(Tensor(a!) acc, Tensor dy, Tensor x, Tensor? grad_scale=None) -> ()", &wgrad_accumulate_);
+  m.def("wgrad_accumulate_supported(Tensor acc, Tensor dy, Tensor x) -> bool", &wgrad_accumulate_ok);
   m.def("wgrad_allreduce_sgd_supported(Tensor w, Tensor dy, Tensor x) -> bool", &wgrad_allreduce_sgd_supported);
   m.def("wgrad_allreduce_sgd_(Tensor(a!) w, Tensor dy, Tensor x, float scale, Tensor? grad_scale=None) -> ()",
         &wgrad_allreduce_sgd_);

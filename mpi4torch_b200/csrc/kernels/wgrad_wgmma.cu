@@ -1,5 +1,5 @@
 // Weight-gradient GEMM on wgmma, optionally fused with the gradient all-reduce and
-// the SGD update.
+// the SGD update, or accumulated into an fp32 gradient buffer.
 //
 //   G[N,K] = dY[Mb,N]^T * X[Mb,K]          (bf16 in, fp32 accumulate in registers)
 //
@@ -50,7 +50,8 @@ constexpr int kMaxUnicastRanks = 3;  // peer-load mode keeps ranks x rows x part
 template <bool FUSED> constexpr int tile_n() { return FUSED ? 128 : 256; }
 
 struct WgradArgs {
-  void* out;            // plain: G [N, K]; fused: unused (the staging buffers live in the heaps of WgradComm)
+  void* out;            // plain: G [N, K] (bf16; fp32 when ACC32); fused: unused (the staging buffers live in
+                        // the heaps of WgradComm)
   int Mb, N, K;
   int ldo;              // leading dimension of out (elements)
   int ksplit;
@@ -294,7 +295,9 @@ __device__ __forceinline__ void comm_reduce_update(const WgradComm& wc, int firs
   asm volatile("bar.sync 1, %0;" ::"n"(kCommThreads));
 }
 
-template <bool FUSED>
+// ACC32 (plain mode only): out is an fp32 [N, K] buffer and the epilogue is out <- fmaf(gscale, G, out), the
+// gradient accumulation of micro-batches.  A compile-time mode, so the other instantiations are unchanged.
+template <bool FUSED, bool ACC32 = false>
 __global__ void __launch_bounds__(kGemmThreads + (FUSED ? kCommWarps * 32 : 0), 1)
 wgrad_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                         const WgradArgs g, const WgradComm wc) {
@@ -369,6 +372,30 @@ wgrad_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
       }
       const float gs = (g.gscale ? __ldg(g.gscale) : 1.0f) * (g.axpy != 0.0f ? g.axpy : 1.0f);
       const bool axpy = !FUSED && g.axpy != 0.0f;
+      if constexpr (ACC32) {
+        // out[r, c] <- fmaf(gs, acc, out[r, c]): ONE rounding per micro-batch (the product is not rounded on its
+        // own), so a contribution far below the buffer's ulp still moves it by its correctly rounded share.
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          const int row = n_blk * BM + wgi * 64 + frag_row(hr);
+          float* orow = reinterpret_cast<float*>(obase) + static_cast<int64_t>(row) * ldo + k_blk * BN;
+          const int cols = min(BN, g.K - k_blk * BN);  // a multiple of 128
+#pragma unroll
+          for (int j0 = 0; j0 < BN / 8; j0 += 8) {
+            if (j0 * 8 >= cols) continue;
+            float2 prev[8];  // the eight column pairs of the row are requested before any is consumed
+#pragma unroll
+            for (int j = 0; j < 8; ++j) prev[j] = *reinterpret_cast<const float2*>(orow + frag_col(j0 + j));
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const float2 o = make_float2(fmaf(gs, acc[4 * (j0 + j) + 2 * hr], prev[j].x),
+                                           fmaf(gs, acc[4 * (j0 + j) + 2 * hr + 1], prev[j].y));
+              *reinterpret_cast<float2*>(orow + frag_col(j0 + j)) = o;
+            }
+          }
+        }
+        continue;
+      }
 #pragma unroll
       for (int hr = 0; hr < 2; ++hr) {
         const int row = n_blk * BM + wgi * 64 + frag_row(hr);
@@ -417,10 +444,10 @@ CUtensorMap make_tmap_mn(const void* base, int64_t rows, int64_t cols, int64_t l
   return make_tmap_bf16_sw128(base, rows, cols, ld, 64, BK);
 }
 
-template <bool FUSED> void configure_w() {
+template <bool FUSED, bool ACC32 = false> void configure_w() {
   static std::once_flag once;
   std::call_once(once, [] {
-    cudaError_t e = cudaFuncSetAttribute(wgrad_bf16_wgmma_kernel<FUSED>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(wgrad_bf16_wgmma_kernel<FUSED, ACC32>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          Tile<tile_n<FUSED>()>::kSmemBytes);
     M4T_CHECK(e == cudaSuccess, "cudaFuncSetAttribute(smem) failed: " << cudaGetErrorString(e));
   });
@@ -464,6 +491,36 @@ void launch_wgrad_bf16(const void* dy, const void* x, void* gout, int64_t Mb, in
   cudaError_t e = cudaGetLastError();
   M4T_CHECK(e == cudaSuccess, "wgrad_bf16 launch failed: " << cudaGetErrorString(e));
   note_kernel_launch(axpy != 0.0f ? "wgrad_sgd_epilogue" : "wgrad");
+}
+
+bool wgrad_accumulate_supported(int64_t Mb, int64_t N, int64_t K, const void* dy, const void* x, const float* acc,
+                                int64_t ldy, int64_t ldx) {
+  return wgrad_bf16_supported(Mb, N, K, dy, x, acc, ldy, ldx, K);
+}
+
+void launch_wgrad_accumulate(const void* dy, const void* x, float* acc, int64_t Mb, int64_t N, int64_t K, int64_t ldy,
+                             int64_t ldx, int sm_count, cudaStream_t stream, const float* gscale) {
+  M4T_CHECK(wgrad_accumulate_supported(Mb, N, K, dy, x, acc, ldy, ldx),
+            "unsupported wgrad_accumulate shape/alignment (N % 128, K % 128, batch % 64, 16-byte aligned operands)");
+  const CUtensorMap ta = make_tmap_mn(dy, Mb, N, ldy);
+  const CUtensorMap tb = make_tmap_mn(x, Mb, K, ldx);
+  WgradArgs g{};
+  g.out = acc;
+  g.Mb = static_cast<int>(Mb);
+  g.N = static_cast<int>(N);
+  g.K = static_cast<int>(K);
+  g.ldo = static_cast<int>(K);
+  g.ksplit = 1;
+  g.gscale = gscale;
+  g.axpy = 0.0f;
+  constexpr int BN = tile_n<false>();
+  const int tiles = static_cast<int>((N / BM) * ((K + BN - 1) / BN));
+  const int grid = std::max(1, std::min(tiles, sm_count));
+  configure_w<false, true>();
+  wgrad_bf16_wgmma_kernel<false, true><<<grid, kGemmThreads, Tile<BN>::kSmemBytes, stream>>>(ta, tb, g, WgradComm{});
+  cudaError_t e = cudaGetLastError();
+  M4T_CHECK(e == cudaSuccess, "wgrad_accumulate launch failed: " << cudaGetErrorString(e));
+  note_kernel_launch("wgrad_accumulate");
 }
 
 int64_t fused_wgrad_tiles(int64_t N, int64_t K) { return (N / BM) * (K / tile_n<true>()); }

@@ -12,13 +12,18 @@ One training step, every rank, written the way the reference's data-parallel exa
                                                one kernel when the optimizer runs in backward)
 
 With ``sgd_in_backward=False`` the weight gets an ordinary ``.grad`` and ``train_step`` applies SGD.
+``train_step(x, t, micro_batches=K)`` with K > 1 accumulates the gradients of K equal chunks of the batch in
+``model.accumulator`` (an :class:`AccumulatedSGD`, fp32 buffers, no parameter-sized collective in backward) and
+then updates once.
 """
 from __future__ import annotations
 
 import torch
 
 import mpi4torch_b200 as m4t
-from mpi4torch_b200.ops import InBackwardSGD, allreduce_linear, dp_linear_mse, in_backward_sgd_supported
+from mpi4torch_b200.models.dp_mlp import accumulated_step
+from mpi4torch_b200.ops import (AccumulatedSGD, InBackwardSGD, allreduce_linear, dp_linear_mse,
+                                in_backward_sgd_supported)
 
 
 class DPLinearModel:
@@ -43,6 +48,7 @@ class DPLinearModel:
         self.fused = fused  # Allreduce->GEMM in one kernel when the NVLS path is up
         self.sgd_in_backward = sgd_in_backward  # fused wgrad -> reduce-scatter -> SGD -> multicast in backward
         self.optimizer = InBackwardSGD(lr, prefetch=prefetch, assume_replicated=assume_replicated)
+        self.accumulator = AccumulatedSGD(lr)  # train_step(..., micro_batches > 1)
         self._opt_ok = {}
 
     # ------------------------------------------------------------------ graph construction
@@ -67,8 +73,17 @@ class DPLinearModel:
                               optimizer=opt, allow_fused=self.fused)
         return self.comm.Allreduce(local, m4t.MPI_SUM)
 
-    def train_step(self, x: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
-        """forward + backward + SGD update through the autograd graph; returns the (global) loss."""
+    def _local_loss(self, x, target, loss_scale, accumulator):
+        return dp_linear_mse(x, self.weight, target, self.comm, loss_scale=loss_scale, allow_fused=self.fused,
+                             accumulator=accumulator)
+
+    def train_step(self, x: torch.Tensor, target: torch.Tensor, micro_batches: int = 1) -> torch.Tensor:
+        """forward + backward + SGD update through the autograd graph; returns the (global) loss.
+
+        ``micro_batches`` = K > 1: K forwards and backwards over equal chunks of this rank's batch (K must divide it)
+        into ``self.accumulator``, then one update; the loss returned is the whole batch's."""
+        if micro_batches != 1:
+            return accumulated_step(self.comm, self.accumulator, self._local_loss, x, target, micro_batches)
         value = self.loss(x, target)
         value.backward()
         if self.weight.grad is not None:  # the optimizer did not run inside backward

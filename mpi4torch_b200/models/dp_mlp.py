@@ -15,6 +15,13 @@ forward came before another backward's weight update raises ``RuntimeError``, be
 overwritten.  So summing two losses and calling ``backward()`` once raises, after applying one of the two updates.  Biases are fp32 when the weights are 16-bit: a bf16 bias would lose SGD updates
 below 2^-8 of its value.
 
+``train_step(x, t, micro_batches=K)`` with K > 1 is gradient accumulation: the batch is split into K chunks, each
+chunk's forward and backward add this rank's gradients into the fp32 buffers of ``model.accumulator`` (an
+:class:`AccumulatedSGD`, whatever ``sgd_in_backward`` says) with no parameter-sized collective, and one
+``accumulator.step()`` all-reduces the buffers and updates the parameters.  The accumulator is also the supported
+way to combine several losses into one update: pass ``accumulator=model.accumulator`` to ``dp_mlp_mse``, sum the
+losses, call ``backward()`` once, then ``model.accumulator.step()``.
+
 ``DPMLPClassifier`` is the same model with a softmax cross-entropy loss over integer class labels
 (``dp_mlp_cross_entropy``); only the output layer's forward kernels differ.
 """
@@ -24,11 +31,18 @@ import torch
 import torch.nn.functional as F
 
 import mpi4torch_b200 as m4t
-from mpi4torch_b200.ops import (InBackwardSGD, dp_mlp_cross_entropy, dp_mlp_cross_entropy_supported, dp_mlp_mse,
-                                dp_mlp_mse_supported, mlp_in_backward_sgd_supported)
+from mpi4torch_b200.ops import (AccumulatedSGD, InBackwardSGD, dp_mlp_cross_entropy, dp_mlp_cross_entropy_supported,
+                                dp_mlp_mse, dp_mlp_mse_supported, mlp_in_backward_sgd_supported)
 
 
 class DPMLPModel:
+    """The data-parallel two-layer MLP with an MSE loss (see the module docstring for one step).
+
+    ``model.accumulator`` (an :class:`AccumulatedSGD`) is the supported way to combine several losses into one update:
+    pass ``accumulator=model.accumulator`` to ``dp_mlp_mse``, call ``backward()`` on each loss or on their sum, then
+    ``model.accumulator.step()``.  ``train_step(x, t, micro_batches=K)`` does this for K chunks of one batch.  With the
+    in-backward optimizers, summing two ``loss()`` results and calling ``backward()`` once raises instead."""
+
     def __init__(self, in_features: int, hidden_features: int, out_features: int, comm=None, device="cuda",
                  dtype=torch.bfloat16, lr: float = 1e-4, seed: int = 0, sgd_in_backward: bool = True,
                  prefetch: bool = True):
@@ -47,6 +61,7 @@ class DPMLPModel:
         self.lr = lr
         self.sgd_in_backward = sgd_in_backward
         self.optimizers = (InBackwardSGD(lr, prefetch=prefetch), InBackwardSGD(lr, prefetch=prefetch))
+        self.accumulator = AccumulatedSGD(lr)  # train_step(..., micro_batches > 1)
         self._opt_ok = {}
 
     @staticmethod
@@ -75,15 +90,23 @@ class DPMLPModel:
     def _kernels_supported(self, x: torch.Tensor, target: torch.Tensor) -> bool:
         return dp_mlp_mse_supported(x, self.w1, self.b1, self.w2, self.b2, target, self.comm)
 
+    def _local_loss(self, x, target, loss_scale, optimizers=None, accumulator=None):
+        return dp_mlp_mse(x, self.w1, self.b1, self.w2, self.b2, target, self.comm, loss_scale=loss_scale,
+                          optimizers=optimizers, accumulator=accumulator)
+
     def loss(self, x: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
         """Global mean-squared-error loss as a differentiable one-element tensor."""
         opts = self.optimizers if self._in_backward(x, target) else None
-        local = dp_mlp_mse(x, self.w1, self.b1, self.w2, self.b2, target, self.comm,
-                           loss_scale=1.0 / (x.shape[0] * self.comm.size), optimizers=opts)
+        local = self._local_loss(x, target, 1.0 / (x.shape[0] * self.comm.size), optimizers=opts)
         return self.comm.Allreduce(local, m4t.MPI_SUM)
 
-    def train_step(self, x: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
-        """forward + backward + SGD update through the autograd graph; returns the (global) loss."""
+    def train_step(self, x: torch.Tensor, target: torch.Tensor, micro_batches: int = 1) -> torch.Tensor:
+        """forward + backward + SGD update through the autograd graph; returns the (global) loss.
+
+        ``micro_batches`` = K > 1: K forwards and backwards over equal chunks of this rank's batch (K must divide it)
+        into ``self.accumulator``, then one update; the loss returned is the whole batch's."""
+        if micro_batches != 1:
+            return accumulated_step(self.comm, self.accumulator, self._local_loss, x, target, micro_batches)
         value = self.loss(x, target)
         value.backward()
         if any(p.grad is not None for p in self.parameters()):  # the optimizers did not run inside backward
@@ -95,6 +118,27 @@ class DPMLPModel:
                         p.add_(p.grad, alpha=-self.lr)
                         p.grad = None
         return value.detach().reshape(())
+
+
+def accumulated_step(comm, accumulator: AccumulatedSGD, local_loss, x: torch.Tensor, target: torch.Tensor,
+                     micro_batches: int) -> torch.Tensor:
+    """One SGD step over ``micro_batches`` equal chunks of this rank's batch, accumulated in ``accumulator``:
+    ``local_loss(x_chunk, target_chunk, loss_scale, accumulator=...)`` per chunk with ``loss_scale = 1 / (B * P)``
+    of the WHOLE batch, so the buffers hold the whole batch's gradient; then one ``accumulator.step()``.  Returns
+    the global loss of the whole batch (the sum of the chunks' global losses)."""
+    B = x.shape[0]
+    K = int(micro_batches)
+    if K < 1 or B % K != 0:
+        raise ValueError(f"mpi4torch_b200: micro_batches={micro_batches} must be a positive divisor of the batch "
+                         f"size {B}")
+    loss_scale = 1.0 / (B * comm.size)
+    total = None
+    for xc, tc in zip(x.split(B // K), target.split(B // K)):
+        value = comm.Allreduce(local_loss(xc, tc, loss_scale, accumulator=accumulator), m4t.MPI_SUM)
+        value.backward()
+        total = value.detach() if total is None else total + value.detach()
+    accumulator.step()
+    return total.reshape(())
 
 
 class DPMLPClassifier(DPMLPModel):
@@ -122,12 +166,14 @@ class DPMLPClassifier(DPMLPModel):
     def _kernels_supported(self, x: torch.Tensor, labels: torch.Tensor) -> bool:
         return dp_mlp_cross_entropy_supported(x, self.w1, self.b1, self.w2, self.b2, labels, self.comm)
 
+    def _local_loss(self, x, labels, loss_scale, optimizers=None, accumulator=None):
+        return dp_mlp_cross_entropy(x, self.w1, self.b1, self.w2, self.b2, labels, self.comm, loss_scale=loss_scale,
+                                    ignore_index=self.ignore_index, optimizers=optimizers, accumulator=accumulator)
+
     def loss(self, x: torch.Tensor, labels: torch.Tensor) -> torch.Tensor:
         """Global cross-entropy loss (sum over non-ignored rows / (B * P)) as a differentiable one-element tensor."""
         opts = self.optimizers if self._in_backward(x, labels) else None
-        local = dp_mlp_cross_entropy(x, self.w1, self.b1, self.w2, self.b2, labels, self.comm,
-                                     loss_scale=1.0 / (x.shape[0] * self.comm.size), ignore_index=self.ignore_index,
-                                     optimizers=opts)
+        local = self._local_loss(x, labels, 1.0 / (x.shape[0] * self.comm.size), optimizers=opts)
         return self.comm.Allreduce(local, m4t.MPI_SUM)
 
     @torch.no_grad()

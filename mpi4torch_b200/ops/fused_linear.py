@@ -13,7 +13,9 @@ csrc/extension.cpp:254-308: forward communicates, backward runs the adjoint comm
   the adjoint Allreduce of the gradient.  With an :class:`InBackwardSGD` attached, backward is ONE
   kernel: wgrad GEMM -> reduce-scatter through the NVSwitch -> ``W += -lr/size * sum`` -> multicast of
   the new weights (-> Allreduce of the new weights for the next forward), i.e. the optimizer step runs
-  inside ``loss.backward()`` and the weight receives no ``.grad``.
+  inside ``loss.backward()`` and the weight receives no ``.grad``.  With an :class:`AccumulatedSGD`
+  attached, backward adds this rank's gradient into an fp32 buffer (the wgrad kernel's accumulating
+  epilogue) and issues no collective; ``step()`` all-reduces the buffers and updates once.
 
 Elsewhere (CPU tensors, other dtypes/shapes, communicators created by ``Split``) the same math runs
 as the composition ``F.linear(x, AllreduceFused(W, SUM, 1/size))``.
@@ -75,6 +77,121 @@ class InBackwardSGD:
 
     def invalidate(self) -> None:
         self._wavg = None
+
+
+class AccumulatedSGD:
+    """Plain SGD over gradients accumulated across micro-batches (gradient accumulation).
+
+    The nodes (``dp_linear_mse``, ``dp_mlp_mse``, ``dp_mlp_cross_entropy``) take it as ``accumulator=``.  Their
+    backward adds THIS rank's gradient of its local loss into a per-parameter buffer and issues no collective: on the
+    kernel path ``wgrad_accumulate_`` (the wgrad GEMM with an fp32 read-modify-write epilogue) for the weights and
+    ``buf += column_sum(...)`` for the biases; elsewhere a small autograd node adds the gradient of the parameter
+    average.  The parameters get no ``.grad``, and a parameter with ``requires_grad=False`` gets no buffer.
+
+    A buffer is fp32 for a 16-bit parameter and has the parameter's dtype otherwise.  It is allocated at the first
+    backward that reaches its parameter and zeroed by :meth:`step`, which applies, per buffered parameter,
+    ``p += AllreduceFused(buf, SUM, -lr / P)``: one parameter-sized collective per parameter and step, summed in a
+    fixed order, so every rank ends with the same bits.
+
+    The parameter averages ``mean_ranks(p)`` that the forwards read are computed once per step (by the first
+    forward) and reused by the later forwards of the same step.  ``updates`` counts the calls of :meth:`step`; a
+    backward whose forward came before the last :meth:`step` raises ``RuntimeError``.  Several forwards before one
+    backward (``(loss(xa) + loss(xb)).backward()``) are allowed and give the buffers of separate backwards.
+    """
+
+    def __init__(self, lr: float):
+        self.lr = float(lr)
+        self.updates = 0
+        self._bufs = {}  # id(param) -> (param, buffer, comm)
+        self._avgs = {}  # id(param) -> (param, version, average)
+
+    def buffer(self, param: torch.Tensor, comm) -> torch.Tensor:
+        """The gradient buffer of ``param`` (allocated zeroed at the first call)."""
+        entry = self._bufs.get(id(param))
+        if entry is None or entry[0] is not param:
+            dtype = torch.float32 if param.dtype in (torch.bfloat16, torch.float16) else param.dtype
+            entry = (param, torch.zeros(param.shape, dtype=dtype, device=param.device), comm)
+            self._bufs[id(param)] = entry
+        return entry[1]
+
+    def buffers(self):
+        """``(param, buffer)`` of every parameter that has a buffer."""
+        return [(p, b) for p, b, _ in self._bufs.values()]
+
+    def average(self, comm, param: torch.Tensor, compute=None) -> torch.Tensor:
+        """``mean_ranks(param)`` (detached) for this step: computed by ``compute()`` (default ``AllreduceFused``;
+        the parameter itself at one rank) at the first call after a :meth:`step`, reused until the next one or
+        until the parameter's version counter shows an in-place change."""
+        hit = self.cached_average(param)
+        if hit is not None:
+            return hit
+        if compute is not None:
+            avg = compute()
+        elif comm.size == 1:
+            avg = param.detach()
+        else:
+            avg = comm.AllreduceFused(param.detach(), m4t.MPI_SUM, 1.0 / comm.size, None)
+        self.keep_average(param, avg)
+        return self._avgs[id(param)][2]
+
+    def cached_average(self, param: torch.Tensor) -> Optional[torch.Tensor]:
+        entry = self._avgs.get(id(param))
+        if entry is None or entry[0] is not param or entry[1] != param._version:
+            return None
+        return entry[2]
+
+    def keep_average(self, param: torch.Tensor, avg: torch.Tensor) -> None:
+        """Keep ``avg`` as this step's average of ``param``; it must be a tensor no later call overwrites."""
+        self._avgs[id(param)] = (param, param._version, avg.detach())
+
+    def check_fresh(self, updates_at_forward: int) -> None:
+        if self.updates != updates_at_forward:
+            raise RuntimeError("mpi4torch_b200: AccumulatedSGD.step() ran between this node's forward and its "
+                               "backward, so its saved parameter averages are stale; run the backward of every "
+                               "forward before step()")
+
+    @torch.no_grad()
+    def step(self) -> None:
+        """One SGD update per buffered parameter from the sum of every rank's buffer; zeroes the buffers."""
+        for p, buf, comm in self._bufs.values():
+            upd = comm.AllreduceFused(buf, m4t.MPI_SUM, -self.lr / comm.size, None)
+            p.add_(upd)
+            buf.zero_()
+        self.updates += 1
+        self._avgs.clear()
+
+
+class _AccumulateGrad(torch.autograd.Function):
+    """Identity on the detached parameter average ``avg``; backward adds the incoming gradient into the accumulator's
+    buffer of ``param`` (no collective) and gives ``param`` no gradient.  The composition paths' accumulation."""
+
+    @staticmethod
+    def forward(ctx, param, avg, acc, comm):
+        ctx.acc, ctx.comm, ctx.param, ctx.updates = acc, comm, param, acc.updates
+        return avg.view_as(avg)
+
+    @staticmethod
+    def backward(ctx, grad):
+        ctx.acc.check_fresh(ctx.updates)
+        buf = ctx.acc.buffer(ctx.param, ctx.comm)
+        buf.add_(grad.to(buf.dtype))
+        return None, None, None, None
+
+
+def accumulated_average(acc: AccumulatedSGD, comm, param: torch.Tensor) -> torch.Tensor:
+    """This step's ``mean_ranks(param)`` whose gradient goes into ``acc`` (composition paths).  At one rank it is a
+    copy: ``step()`` updates the parameter in place while a stale node may still hold the average."""
+    avg = acc.average(comm, param, (lambda: param.detach().clone()) if comm.size == 1 else None)
+    return _AccumulateGrad.apply(param, avg, acc, comm) if param.requires_grad else avg
+
+
+def _wgrad_accumulate(buf: torch.Tensor, gy: torch.Tensor, x: torch.Tensor, gscale: Optional[torch.Tensor]) -> None:
+    """buf += gscale * gy^T @ x, on the accumulating wgrad kernel when it applies."""
+    if buf.is_cuda and m4t.cuda_backend_ready() and _ops().wgrad_accumulate_supported(buf, gy, x):
+        _ops().wgrad_accumulate_(buf, gy, x, gscale)
+        return
+    g = gy.t().to(buf.dtype) @ x.to(buf.dtype)
+    buf.add_(g if gscale is None else g * gscale.to(buf.dtype))
 
 
 def _wgrad(gy: torch.Tensor, x: torch.Tensor, gscale: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -191,6 +308,40 @@ class _DPLinearMSE(torch.autograd.Function):
         return gx, gw, None, None, None, None, None
 
 
+class _DPLinearMSEAccumulate(torch.autograd.Function):
+    """:class:`_DPLinearMSE` with an :class:`AccumulatedSGD`: the forward reads this step's average of the weight (the
+    first forward of a step computes and keeps it), and backward adds ``g * dy^T x`` into the accumulator's fp32 buffer
+    (``wgrad_accumulate_``) with no collective; the weight gets no ``.grad``."""
+
+    @staticmethod
+    def forward(ctx, x, weight, target, comm_holder, loss_scale, acc, allow_fused):
+        comm = comm_holder[0]
+        ops = _ops()
+        w_avg = acc.cached_average(weight)
+        if w_avg is not None:
+            dy, local = ops.linear_mse_forward_local(x, w_avg, target, loss_scale, 2.0 * loss_scale)
+        else:
+            dy, local, w_avg = ops.linear_mse_forward(x, weight, target, 1.0 / comm.size, loss_scale, 2.0 * loss_scale,
+                                                      allow_fused)
+            # with P > 1 the fused forward's w_avg lives in a two-deep symmetric buffer: keep a copy
+            acc.keep_average(weight, w_avg if comm.size == 1 else w_avg.clone())
+        ctx.save_for_backward(dy, x, w_avg.clone() if ctx.needs_input_grad[0] else None)
+        ctx.comm, ctx.acc, ctx.weight, ctx.acc_updates = comm, acc, weight, acc.updates
+        return local
+
+    @staticmethod
+    def backward(ctx, g):
+        ctx.acc.check_fresh(ctx.acc_updates)
+        dy, x, w_avg = ctx.saved_tensors
+        g = g.reshape(1).to(torch.float32)
+        gx = None
+        if ctx.needs_input_grad[0]:
+            gx = _dgrad(dy, w_avg) * g.to(dy.dtype)
+        if ctx.needs_input_grad[1]:
+            _wgrad_accumulate(ctx.acc.buffer(ctx.weight, ctx.comm), dy, x, g)
+        return gx, None, None, None, None, None, None
+
+
 def dp_linear_mse_supported(x: torch.Tensor, weight: torch.Tensor, target: torch.Tensor, comm) -> bool:
     return (comm.is_world and x.is_cuda and x.dim() == 2 and target.dim() == 2 and x.dtype == torch.bfloat16
             and target.dtype == torch.bfloat16 and weight.dtype == torch.bfloat16 and weight.is_cuda
@@ -210,13 +361,25 @@ def in_backward_sgd_supported(x: torch.Tensor, weight: torch.Tensor, comm) -> bo
 
 
 def dp_linear_mse(x: torch.Tensor, weight: torch.Tensor, target: torch.Tensor, comm=None, *, loss_scale: float,
-                  optimizer: Optional[InBackwardSGD] = None, allow_fused: bool = True) -> torch.Tensor:
+                  optimizer: Optional[InBackwardSGD] = None, allow_fused: bool = True,
+                  accumulator: Optional[AccumulatedSGD] = None) -> torch.Tensor:
     """``loss_scale * sum((x @ mean_ranks(weight)^T - target)^2)`` of THIS rank's batch as a
     differentiable one-element fp32 tensor; sum it over ranks with ``comm.Allreduce``.
 
     ``optimizer``: an :class:`InBackwardSGD` makes ``backward`` apply the SGD step itself (fused
-    into the gradient reduce-scatter); the weight then receives no ``.grad``."""
+    into the gradient reduce-scatter); the weight then receives no ``.grad``.
+    ``accumulator``: an :class:`AccumulatedSGD` makes ``backward`` add this rank's gradient into its buffer
+    (no collective, no ``.grad``); ``accumulator.step()`` updates the weight.  Not combinable with ``optimizer``."""
     c = m4t.COMM_WORLD if comm is None else comm
+    if accumulator is not None and optimizer is not None:
+        raise ValueError("mpi4torch_b200: dp_linear_mse takes either optimizer= or accumulator=, not both")
+    if accumulator is not None:
+        if dp_linear_mse_supported(x, weight, target, c):
+            return _DPLinearMSEAccumulate.apply(x, weight, target, [c], float(loss_scale), accumulator,
+                                                bool(allow_fused))
+        y = F.linear(x, accumulated_average(accumulator, c, weight))
+        acc = torch.float64 if y.dtype == torch.float64 else torch.float32
+        return ((y.to(acc) - target.to(acc)).square().sum() * loss_scale).reshape(1)
     if dp_linear_mse_supported(x, weight, target, c):
         if optimizer is not None and not in_backward_sgd_supported(x, weight, c):
             raise RuntimeError("mpi4torch_b200: InBackwardSGD needs a bf16 CUDA weight from symmetric_empty() on the "

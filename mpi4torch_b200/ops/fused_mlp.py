@@ -10,7 +10,9 @@ Backward is the GELU-backward GEMM (dz, with its column-sum partials), the two w
 deterministic column-sum reduce for the biases.  With :class:`InBackwardSGD` optimizers the weights are
 updated inside backward by the wgrad kernels (with P > 1: reduce-scatter -> SGD -> multicast -> average of
 the new weights for the next forward, one kernel per weight) and the biases by ``allreduce_axpy_``; the
-parameters then receive no ``.grad``.
+parameters then receive no ``.grad``.  With an :class:`AccumulatedSGD` backward instead adds this rank's gradients
+into fp32 buffers (``wgrad_accumulate_`` for the weights, column sums for the biases) with no collective, and the
+forwards of one step share the parameter averages computed by its first forward.
 
 ``dp_mlp_cross_entropy(x, W1, b1, W2, b2, labels, ...)``  loss_local = loss_scale * sum_rows CE(y, labels)
     The same node with a softmax cross-entropy output layer: the second GEMM stores the bf16 logits and per-tile
@@ -30,7 +32,7 @@ import torch.nn.functional as F
 
 import mpi4torch_b200 as m4t
 
-from .fused_linear import InBackwardSGD, _ops
+from .fused_linear import AccumulatedSGD, InBackwardSGD, _ops, accumulated_average
 
 
 def _average(comm, p: torch.Tensor) -> torch.Tensor:
@@ -50,22 +52,27 @@ def _update_weight(ops, comm, opt: InBackwardSGD, weight, dy, x, g) -> None:
         opt.remember(weight, None)
 
 
-def _mlp_forward(ctx, x, w1, b1, w2, b2, comm, opts, output_layer):
-    """Forward of the MLP nodes up to the loss: the parameter averages (or the prefetched ones), the bias + GELU GEMM,
-    then ``output_layer(ops, h, w2_avg, b2_avg) -> (dy, loss, dy_part)``, which stores dL/dy and its column-sum
-    partials.  Saves what :meth:`_DPMLPMSE.backward` reads."""
+def _mlp_forward(ctx, x, w1, b1, w2, b2, comm, opts, output_layer, acc=None):
+    """Forward of the MLP nodes up to the loss: the parameter averages (the prefetched ones, or with an accumulator
+    this step's), the bias + GELU GEMM, then ``output_layer(ops, h, w2_avg, b2_avg) -> (dy, loss, dy_part)``, which
+    stores dL/dy and its column-sum partials.  Saves what :meth:`_DPMLPMSE.backward` reads."""
     ops = _ops()
-    w1_avg = opts[0].take_prefetched(w1) if opts is not None else None
-    w2_avg = opts[1].take_prefetched(w2) if opts is not None else None
-    w1_avg = _average(comm, w1) if w1_avg is None else w1_avg
-    w2_avg = _average(comm, w2) if w2_avg is None else w2_avg
-    h, z = ops.linear_bias_gelu_forward(x, w1_avg, _average(comm, b1))
-    dy, local, dy_part = output_layer(ops, h, w2_avg, _average(comm, b2))
+    if acc is not None:
+        w1_avg, b1_avg, w2_avg, b2_avg = (acc.average(comm, p) for p in (w1, b1, w2, b2))
+    else:
+        w1_avg = opts[0].take_prefetched(w1) if opts is not None else None
+        w2_avg = opts[1].take_prefetched(w2) if opts is not None else None
+        w1_avg = _average(comm, w1) if w1_avg is None else w1_avg
+        w2_avg = _average(comm, w2) if w2_avg is None else w2_avg
+        b1_avg, b2_avg = _average(comm, b1), _average(comm, b2)
+    h, z = ops.linear_bias_gelu_forward(x, w1_avg, b1_avg)
+    dy, local, dy_part = output_layer(ops, h, w2_avg, b2_avg)
     ctx.save_for_backward(x, h, z, dy, w1_avg, w2_avg, dy_part)
-    ctx.comm, ctx.opts, ctx.params = comm, opts, (w1, b1, w2, b2)
+    ctx.comm, ctx.opts, ctx.params, ctx.acc = comm, opts, (w1, b1, w2, b2), acc
     # w1_avg / w2_avg are the weights themselves (P = 1) or the prefetch buffers (P > 1), which the next in-backward
     # update rewrites without bumping torch's version counter: backward checks these counts instead
     ctx.opt_updates = None if opts is None else (opts[0].updates, opts[1].updates)
+    ctx.acc_updates = None if acc is None else acc.updates
     return local
 
 
@@ -74,14 +81,16 @@ class _DPMLPMSE(torch.autograd.Function):
     into the kernels' epilogues (never read on the host)."""
 
     @staticmethod
-    def forward(ctx, x, w1, b1, w2, b2, target, comm_holder, loss_scale, opts):
+    def forward(ctx, x, w1, b1, w2, b2, target, comm_holder, loss_scale, opts, acc=None):
         def output_layer(ops, h, w2_avg, b2_avg):
             return ops.linear_bias_mse_forward_local(h, w2_avg, b2_avg, target, loss_scale, 2.0 * loss_scale)
 
-        return _mlp_forward(ctx, x, w1, b1, w2, b2, comm_holder[0], opts, output_layer)
+        return _mlp_forward(ctx, x, w1, b1, w2, b2, comm_holder[0], opts, output_layer, acc)
 
     @staticmethod
     def backward(ctx, g):
+        if ctx.acc is not None:
+            return _accumulate_backward(ctx, g)
         x, h, z, dy, w1_avg, w2_avg, dy_part = ctx.saved_tensors
         comm, opts = ctx.comm, ctx.opts
         w1, b1, w2, b2 = ctx.params
@@ -127,7 +136,31 @@ class _DPMLPMSE(torch.autograd.Function):
                 gb2 = comm.AllreduceFused(db2, m4t.MPI_SUM, 1.0 / comm.size, None)
             if need[2]:
                 gb1 = comm.AllreduceFused(db1, m4t.MPI_SUM, 1.0 / comm.size, None)
-        return gx, gw1, gb1, gw2, gb2, None, None, None, None
+        return gx, gw1, gb1, gw2, gb2, None, None, None, None, None
+
+
+def _accumulate_backward(ctx, g):
+    """Backward of the MLP nodes with an :class:`AccumulatedSGD`: this rank's gradients of the parameter averages
+    are added into the accumulator's buffers, with no collective; only ``x`` gets a gradient.  The averages are this
+    step's, and nothing overwrites them before ``step()``, so the order of the reads does not matter here."""
+    comm, acc = ctx.comm, ctx.acc
+    acc.check_fresh(ctx.acc_updates)  # first: at one rank the saved averages are the parameters that step() updated
+    x, h, z, dy, w1_avg, w2_avg, dy_part = ctx.saved_tensors
+    w1, b1, w2, b2 = ctx.params
+    ops = _ops()
+    g = g.reshape(1).to(torch.float32)
+    need = ctx.needs_input_grad
+    dz, dz_part = ops.gemm_nn_gelu_backward(dy, w2_avg, z, g)
+    if need[3]:
+        ops.wgrad_accumulate_(acc.buffer(w2, comm), dy, h, g)
+    if need[1]:
+        ops.wgrad_accumulate_(acc.buffer(w1, comm), dz, x, None)
+    if need[4]:
+        acc.buffer(b2, comm).add_(ops.column_sum(dy_part, g))
+    if need[2]:
+        acc.buffer(b1, comm).add_(ops.column_sum(dz_part, None))
+    gx = ops.gemm_bf16_nn(dz, w1_avg) if need[0] else None
+    return gx, None, None, None, None, None, None, None, None, None
 
 
 class _DPMLPCrossEntropy(_DPMLPMSE):
@@ -136,13 +169,13 @@ class _DPMLPCrossEntropy(_DPMLPMSE):
     partials, so the backward is inherited unchanged.  ``loss_args`` is ``(loss_scale, ignore_index)``."""
 
     @staticmethod
-    def forward(ctx, x, w1, b1, w2, b2, labels, comm_holder, loss_args, opts):
+    def forward(ctx, x, w1, b1, w2, b2, labels, comm_holder, loss_args, opts, acc=None):
         loss_scale, ignore_index = loss_args
 
         def output_layer(ops, h, w2_avg, b2_avg):
             return ops.linear_bias_xent_forward_local(h, w2_avg, b2_avg, labels, loss_scale, loss_scale, ignore_index)
 
-        return _mlp_forward(ctx, x, w1, b1, w2, b2, comm_holder[0], opts, output_layer)
+        return _mlp_forward(ctx, x, w1, b1, w2, b2, comm_holder[0], opts, output_layer, acc)
 
 
 def _kernel_ops_present() -> bool:
@@ -210,7 +243,8 @@ def mlp_in_backward_sgd_supported(x: torch.Tensor, w1: torch.Tensor, w2: torch.T
 
 def dp_mlp_mse(x: torch.Tensor, w1: torch.Tensor, b1: torch.Tensor, w2: torch.Tensor, b2: torch.Tensor,
                target: torch.Tensor, comm=None, *, loss_scale: float,
-               optimizers: Optional[Sequence[InBackwardSGD]] = None) -> torch.Tensor:
+               optimizers: Optional[Sequence[InBackwardSGD]] = None,
+               accumulator: Optional[AccumulatedSGD] = None) -> torch.Tensor:
     """``loss_scale * sum((MLP(x) - target)^2)`` of THIS rank's batch as a differentiable one-element fp32
     tensor, with every parameter averaged over ranks; sum it over ranks with ``comm.Allreduce``.
 
@@ -221,18 +255,24 @@ def dp_mlp_mse(x: torch.Tensor, w1: torch.Tensor, b1: torch.Tensor, w2: torch.Te
       * run one backward per forward.  Backward reads the weights (or their prefetched averages) as they were at
         this node's forward, and another node's backward updates them in place, so a node whose weights were
         updated since its forward raises ``RuntimeError`` instead of computing its gradients from the new ones.
-        For example ``(model.loss(xa, ta) + model.loss(xb, tb)).backward()`` raises after applying one update."""
+        For example ``(model.loss(xa, ta) + model.loss(xb, tb)).backward()`` raises after applying one update.
+
+    ``accumulator``: an :class:`AccumulatedSGD` makes ``backward`` add this rank's gradients into its buffers instead
+    (no collective, no ``.grad``, frozen parameters skipped); ``accumulator.step()`` then applies one update.  Several
+    forwards may precede one backward in this mode.  It cannot be combined with ``optimizers``."""
     c = m4t.COMM_WORLD if comm is None else comm
+    _check_one_optimizer("dp_mlp_mse", optimizers, accumulator)
     if dp_mlp_mse_supported(x, w1, b1, w2, b2, target, c):
         optimizers = _kernel_optimizers("dp_mlp_mse", optimizers, x, w1, w2, c)
-        return _DPMLPMSE.apply(x, w1, b1, w2, b2, target, [c], float(loss_scale), optimizers)
-    y, acc = _composition(x, w1, b1, w2, b2, c, optimizers)
+        return _DPMLPMSE.apply(x, w1, b1, w2, b2, target, [c], float(loss_scale), optimizers, accumulator)
+    y, acc = _composition(x, w1, b1, w2, b2, c, optimizers, accumulator)
     return ((y.to(acc) - target.to(acc)).square().sum() * loss_scale).reshape(1)
 
 
 def dp_mlp_cross_entropy(x: torch.Tensor, w1: torch.Tensor, b1: torch.Tensor, w2: torch.Tensor, b2: torch.Tensor,
                          labels: torch.Tensor, comm=None, *, loss_scale: float, ignore_index: int = -100,
-                         optimizers: Optional[Sequence[InBackwardSGD]] = None) -> torch.Tensor:
+                         optimizers: Optional[Sequence[InBackwardSGD]] = None,
+                         accumulator: Optional[AccumulatedSGD] = None) -> torch.Tensor:
     """``loss_scale * sum_rows cross_entropy(MLP(x), labels)`` of THIS rank's batch (``F.cross_entropy`` with
     ``reduction="sum"``) as a differentiable one-element fp32 tensor, with every parameter averaged over ranks;
     sum it over ranks with ``comm.Allreduce``.  ``labels``: one int64 class index per row of ``x``.  A row labelled
@@ -242,17 +282,24 @@ def dp_mlp_cross_entropy(x: torch.Tensor, w1: torch.Tensor, b1: torch.Tensor, w2
     The softmax is taken over the bf16 logits ``bf16(h @ W2^T + b2)``.  ``optimizers`` as in :func:`dp_mlp_mse`,
     with the same two rules: frozen parameters are not updated, and one backward per forward.
     The kernels need C % 128 == 0: pad the classes to the next multiple of 128 and give the padded classes bias
-    ``-inf``, which gives them probability 0 and gradient 0, so their bias stays ``-inf``."""
+    ``-inf``, which gives them probability 0 and gradient 0, so their bias stays ``-inf``.
+    ``accumulator`` as in :func:`dp_mlp_mse`."""
     if not (labels.dim() == 1 and labels.dtype == torch.int64 and x.dim() == 2 and labels.shape[0] == x.shape[0]):
         raise ValueError(f"mpi4torch_b200: dp_mlp_cross_entropy needs int64 labels of shape ({x.shape[0]},), got "
                          f"{labels.dtype} of shape {tuple(labels.shape)}")
     c = m4t.COMM_WORLD if comm is None else comm
+    _check_one_optimizer("dp_mlp_cross_entropy", optimizers, accumulator)
     if dp_mlp_cross_entropy_supported(x, w1, b1, w2, b2, labels, c):
         optimizers = _kernel_optimizers("dp_mlp_cross_entropy", optimizers, x, w1, w2, c)
         return _DPMLPCrossEntropy.apply(x, w1, b1, w2, b2, labels, [c], (float(loss_scale), int(ignore_index)),
-                                        optimizers)
-    y, acc = _composition(x, w1, b1, w2, b2, c, optimizers)
+                                        optimizers, accumulator)
+    y, acc = _composition(x, w1, b1, w2, b2, c, optimizers, accumulator)
     return (F.cross_entropy(y.to(acc), labels, reduction="sum", ignore_index=ignore_index) * loss_scale).reshape(1)
+
+
+def _check_one_optimizer(name, optimizers, accumulator):
+    if optimizers is not None and accumulator is not None:
+        raise ValueError(f"mpi4torch_b200: {name} takes either optimizers= or accumulator=, not both")
 
 
 def _kernel_optimizers(name, optimizers, x, w1, w2, c):
@@ -266,12 +313,16 @@ def _kernel_optimizers(name, optimizers, x, w1, w2, c):
     return tuple(optimizers)
 
 
-def _composition(x, w1, b1, w2, b2, c, optimizers):
-    """Off the kernel path: the MLP output ``y`` as the torch composition on ``AllreduceFused`` averages, and the
-    dtype the loss accumulates in (fp32; fp64 inputs stay fp64)."""
+def _composition(x, w1, b1, w2, b2, c, optimizers, accumulator=None):
+    """Off the kernel path: the MLP output ``y`` as the torch composition on ``AllreduceFused`` averages (with an
+    accumulator: this step's averages, whose gradients go into its buffers), and the dtype the loss accumulates in
+    (fp32; fp64 inputs stay fp64)."""
     if optimizers is not None:
         raise RuntimeError("mpi4torch_b200: InBackwardSGD is only available on the CUDA kernel path")
-    avg = lambda p: c.AllreduceFused(p, m4t.MPI_SUM, 1.0 / c.size, None)  # noqa: E731
+    if accumulator is not None:
+        avg = lambda p: accumulated_average(accumulator, c, p)  # noqa: E731
+    else:
+        avg = lambda p: c.AllreduceFused(p, m4t.MPI_SUM, 1.0 / c.size, None)  # noqa: E731
     acc = torch.float64 if x.dtype == torch.float64 else torch.float32
     h = F.gelu(F.linear(x, avg(w1), avg(b1).to(x.dtype)), approximate="tanh")
     return F.linear(h, avg(w2), avg(b2).to(h.dtype)), acc
