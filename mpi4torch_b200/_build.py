@@ -38,6 +38,7 @@ _SOURCES = [
     "kernels/p2p.cu",
     "kernels/gemm_wgmma.cu",
     "kernels/wgrad_wgmma.cu",
+    "kernels/gemm_fp8.cu",
     "api/comm_raw.cpp",
     "api/autograd_ops.cpp",
     "api/fused_ops.cpp",

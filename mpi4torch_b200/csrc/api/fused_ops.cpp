@@ -444,9 +444,150 @@ Tensor column_sum(const Tensor& partials, const c10::optional<Tensor>& grad_scal
   return out;
 }
 
+// ---- FP8 linear layer (gemm_fp8.cu) ------------------------------------------------------------------------------
+bool fp8_e5m2(c10::string_view fmt) {
+  TORCH_CHECK(fmt == "e4m3" || fmt == "e5m2", "mpi4torch_b200: the fp8 format must be 'e4m3' or 'e5m2'");
+  return fmt == "e5m2";
+}
+
+bool is_fp8(const Tensor& t) { return t.scalar_type() == at::kFloat8_e4m3fn || t.scalar_type() == at::kFloat8_e5m2; }
+
+bool scalar_ok(const Tensor& s, const Tensor& like) {
+  return s.is_cuda() && s.device() == like.device() && s.scalar_type() == at::kFloat && s.numel() == 1;
+}
+
+// (q, qt, scale_inv): q = fp8(x * s) [rows, cols] when rowwise, qt = its transpose [cols, rows] when transposed (each
+// contiguous, or None), scale_inv = 1/s as a device fp32 [1].  s is the power of two of amax (DESIGN §4.4): of max|x|,
+// computed here, or of a given device amax (fp32 [1]).
+std::tuple<Tensor, Tensor, Tensor> quantize_fp8(const Tensor& x, c10::string_view fmt, bool rowwise, bool transposed,
+                                                const c10::optional<Tensor>& amax) {
+  const bool e5m2 = fp8_e5m2(fmt);
+  TORCH_CHECK(x.is_cuda() && x.dim() == 2 && x.scalar_type() == at::kBFloat16 && x.stride(1) == 1 && x.numel() > 0,
+              "mpi4torch_b200: quantize_fp8 needs a non-empty 2-d bf16 CUDA tensor with unit inner stride");
+  TORCH_CHECK(rowwise || transposed, "mpi4torch_b200: quantize_fp8 needs rowwise or transposed");
+  const bool given = amax.has_value() && amax->defined();
+  TORCH_CHECK(!given || (scalar_ok(*amax, x) && amax->is_contiguous()),
+              "mpi4torch_b200: amax must be a one-element fp32 tensor on x's device");
+  c10::cuda::CUDAGuard guard(x.device());
+  cudaStream_t stream = c10::cuda::getCurrentCUDAStream(x.device().index()).stream();
+  const auto dt = e5m2 ? at::kFloat8_e5m2 : at::kFloat8_e4m3fn;
+  const int64_t R = x.size(0), C = x.size(1);
+  Tensor q = rowwise ? at::empty({R, C}, x.options().dtype(dt)) : Tensor();
+  Tensor qt = transposed ? at::empty({C, R}, x.options().dtype(dt)) : Tensor();
+  Tensor si = at::empty({1}, x.options().dtype(at::kFloat));
+  std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
+  Tensor am = given ? *amax : at::zeros({1}, x.options().dtype(at::kFloat));
+  auto* bits = reinterpret_cast<unsigned int*>(am.data_ptr<float>());
+  if (!given) launch_quantize_fp8_amax(x.data_ptr(), R, C, x.stride(0), bits, backend().device_comm().sm_count, stream);
+  launch_quantize_fp8_cast(x.data_ptr(), R, C, x.stride(0), e5m2, bits, rowwise ? q.data_ptr() : nullptr,
+                           transposed ? qt.data_ptr() : nullptr, si.data_ptr<float>(), stream);
+  return {q, qt, si};
+}
+
+// The operand rules of the fp8 GEMMs: a [M, K] fp8 (E4M3 or E5M2), b [N, K] E4M3, unit inner strides, K, the row
+// strides and the bases 16-byte aligned, N % 8 == 0, both scale_inv one-element fp32 on the same device; and the MSE
+// target [M, N] (bf16 pairs) or the SGD weight [M, N] (bf16, 16-byte-aligned, row stride % 8) when given.
+bool gemm_fp8_tn_ok(const Tensor& a, const Tensor& b, const Tensor& a_si, const Tensor& b_si,
+                    const c10::optional<Tensor>& target, const c10::optional<Tensor>& w) {
+  if (!(a.is_cuda() && b.is_cuda() && a.device() == b.device() && a.dim() == 2 && b.dim() == 2 && is_fp8(a) &&
+        b.scalar_type() == at::kFloat8_e4m3fn && a.stride(1) == 1 && b.stride(1) == 1 && a.size(1) == b.size(1) &&
+        scalar_ok(a_si, a) && scalar_ok(b_si, a)))
+    return false;
+  if (target.has_value() && target->defined() &&
+      !(target->is_cuda() && target->device() == a.device() && target->dim() == 2 &&
+        target->scalar_type() == at::kBFloat16 && target->stride(1) == 1 && target->size(0) == a.size(0) &&
+        target->size(1) == b.size(0) && epilogue_bf16_pairs_ok(target->data_ptr(), target->stride(0))))
+    return false;
+  const void* c = a.data_ptr();
+  int64_t ldc = b.size(0);
+  if (w.has_value() && w->defined()) {
+    if (!(w->is_cuda() && w->device() == a.device() && w->dim() == 2 && w->scalar_type() == at::kBFloat16 &&
+          w->stride(1) == 1 && w->size(0) == a.size(0) && w->size(1) == b.size(0)))
+      return false;
+    c = w->data_ptr();
+    ldc = w->stride(0);
+  }
+  return World::instance().cuda_ready() &&
+         gemm_fp8_tn_supported(a.size(0), b.size(0), a.size(1), a.data_ptr(), b.data_ptr(), c, a.stride(0), b.stride(0),
+                               ldc);
+}
+
+// C = bf16(grad_scale * a @ b^T * a_scale_inv * b_scale_inv).
+Tensor gemm_fp8_tn(const Tensor& a, const Tensor& b, const Tensor& a_si, const Tensor& b_si,
+                   const c10::optional<Tensor>& grad_scale) {
+  TORCH_CHECK(gemm_fp8_tn_ok(a, b, a_si, b_si, c10::nullopt, c10::nullopt),
+              "mpi4torch_b200: gemm_fp8_tn needs a [M, K] fp8 and b [N, K] float8_e4m3fn CUDA tensors with unit inner "
+              "strides, K and the row strides multiples of 16, 16-byte-aligned bases, N % 8 == 0, and one-element fp32 "
+              "scale_inv tensors on the same device");
+  c10::cuda::CUDAGuard guard(a.device());
+  Tensor c = at::empty({a.size(0), b.size(0)}, a.options().dtype(at::kBFloat16));
+  std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
+  launch_gemm_fp8_tn(a.data_ptr(), a.scalar_type() == at::kFloat8_e5m2, b.data_ptr(), c.data_ptr(), a.size(0), b.size(0),
+                     a.size(1), a.stride(0), b.stride(0), c.stride(0), a_si.data_ptr<float>(), b_si.data_ptr<float>(),
+                     grad_scale_ptr(grad_scale, a), backend().device_comm().sm_count,
+                     c10::cuda::getCurrentCUDAStream(a.device().index()).stream());
+  return c;
+}
+
+// Forward of the fp8 linear layer with the MSE epilogue, against an already averaged weight: (dy, loss[1], dy_amax[1])
+// with y = xq @ wq^T / (s_x s_w), dy = bf16(grad_scale (y - target)), loss = loss_scale * sum((y - target)^2) and
+// dy_amax = max |dy| over the stored bf16 values (fp32), ready for quantize_fp8(dy, "e5m2", amax=dy_amax).
+std::tuple<Tensor, Tensor, Tensor> linear_mse_forward_fp8_local(const Tensor& xq, const Tensor& wq, const Tensor& x_si,
+                                                                const Tensor& w_si, const Tensor& target,
+                                                                double loss_scale, double grad_scale) {
+  TORCH_CHECK(xq.scalar_type() == at::kFloat8_e4m3fn && gemm_fp8_tn_ok(xq, wq, x_si, w_si, target, c10::nullopt),
+              "mpi4torch_b200: linear_mse_forward_fp8_local needs float8_e4m3fn xq [B, K] and wq [N, K] under the "
+              "gemm_fp8_tn operand rules, and a bf16 target [B, N] with unit inner stride, a 4-byte-aligned base and an "
+              "even row stride");
+  c10::cuda::CUDAGuard guard(xq.device());
+  Tensor dy = at::empty({xq.size(0), wq.size(0)}, xq.options().dtype(at::kBFloat16));
+  Tensor loss = at::zeros({1}, xq.options().dtype(at::kFloat));
+  Tensor amax = at::zeros({1}, xq.options().dtype(at::kFloat));
+  MseEpilogue mse;
+  mse.target = target.data_ptr();
+  mse.ldt = target.stride(0);
+  mse.loss_acc = loss.data_ptr<float>();
+  mse.loss_scale = static_cast<float>(loss_scale);
+  mse.grad_scale = static_cast<float>(grad_scale);
+  std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
+  launch_gemm_fp8_mse(xq.data_ptr(), wq.data_ptr(), dy.data_ptr(), xq.size(0), wq.size(0), xq.size(1), xq.stride(0),
+                      wq.stride(0), dy.stride(0), x_si.data_ptr<float>(), w_si.data_ptr<float>(), mse,
+                      reinterpret_cast<unsigned int*>(amax.data_ptr<float>()), backend().device_comm().sm_count,
+                      c10::cuda::getCurrentCUDAStream(xq.device().index()).stream());
+  return {dy, loss, amax};
+}
+
+// w += scale * grad_scale * a @ b^T * a_scale_inv * b_scale_inv, the single-rank SGD step as the fp8 GEMM's epilogue.
+void gemm_fp8_tn_sgd_(Tensor w, const Tensor& a, const Tensor& b, const Tensor& a_si, const Tensor& b_si, double scale,
+                      const c10::optional<Tensor>& grad_scale) {
+  TORCH_CHECK(gemm_fp8_tn_ok(a, b, a_si, b_si, c10::nullopt, w),
+              "mpi4torch_b200: gemm_fp8_tn_sgd_ needs the gemm_fp8_tn operand rules and w a bf16 [M, N] CUDA tensor with "
+              "unit inner stride, a 16-byte-aligned base and a row stride that is a multiple of 8");
+  TORCH_CHECK(scale != 0.0, "mpi4torch_b200: gemm_fp8_tn_sgd_ needs a non-zero scale");
+  c10::cuda::CUDAGuard guard(a.device());
+  std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
+  launch_gemm_fp8_sgd(a.data_ptr(), a.scalar_type() == at::kFloat8_e5m2, b.data_ptr(), w.data_ptr(), a.size(0), b.size(0),
+                      a.size(1), a.stride(0), b.stride(0), w.stride(0), a_si.data_ptr<float>(), b_si.data_ptr<float>(),
+                      static_cast<float>(scale), grad_scale_ptr(grad_scale, a), backend().device_comm().sm_count,
+                      c10::cuda::getCurrentCUDAStream(a.device().index()).stream());
+}
+
 }  // namespace
 
 TORCH_LIBRARY_FRAGMENT(mpi4torch_b200, m) {
+  m.def("quantize_fp8(Tensor x, str fmt, bool rowwise, bool transposed, Tensor? amax=None) -> (Tensor, Tensor, Tensor)",
+        &quantize_fp8);
+  m.def("gemm_fp8_tn_supported(Tensor a, Tensor b, Tensor a_scale_inv, Tensor b_scale_inv, Tensor? target=None, "
+        "Tensor? w=None) -> bool",
+        &gemm_fp8_tn_ok);
+  m.def("gemm_fp8_tn(Tensor a, Tensor b, Tensor a_scale_inv, Tensor b_scale_inv, Tensor? grad_scale=None) -> Tensor",
+        &gemm_fp8_tn);
+  m.def("linear_mse_forward_fp8_local(Tensor xq, Tensor wq, Tensor x_scale_inv, Tensor w_scale_inv, Tensor target, "
+        "float loss_scale, float grad_scale) -> (Tensor, Tensor, Tensor)",
+        &linear_mse_forward_fp8_local);
+  m.def("gemm_fp8_tn_sgd_(Tensor(a!) w, Tensor a, Tensor b, Tensor a_scale_inv, Tensor b_scale_inv, float scale, "
+        "Tensor? grad_scale=None) -> ()",
+        &gemm_fp8_tn_sgd_);
   m.def("linear_bias_gelu_forward(Tensor x, Tensor w, Tensor b) -> (Tensor, Tensor)", &linear_bias_gelu_forward);
   m.def("linear_bias_mse_forward_local(Tensor x, Tensor w, Tensor b, Tensor target, float loss_scale, float grad_scale) "
         "-> (Tensor, Tensor, Tensor)",

@@ -200,6 +200,33 @@ void launch_fused_wgrad_update(const DeviceComm& dc, const void* dy, const void*
 // device word at that heap offset (advanced by the kernel): no host-side step state, graph-capturable.
 // wavg_off >= 0: additionally leaves (1/P) * sum_ranks W_new in the bf16 [N,K] buffer at that heap
 // offset on every rank (the parameter all-reduce of the NEXT forward, run under this GEMM).
+
+// ---- FP8 training of the linear layer (gemm_fp8.cu, DESIGN §4.4) ---------------------------------------------
+// Per-tensor power-of-two scaling: amax of a bf16 [rows, cols] matrix (leading dimension ld) -> *amax_bits (the bit
+// pattern of the fp32 amax; zeroed by the caller, atomicMax), then q = fp8(v * s) row-major [rows, cols] and/or
+// qt = q^T [cols, rows] (either may be null; both contiguous), and *scale_inv = 1/s.
+void launch_quantize_fp8_amax(const void* x, int64_t rows, int64_t cols, int64_t ld, unsigned int* amax_bits,
+                              int sm_count, cudaStream_t stream);
+void launch_quantize_fp8_cast(const void* x, int64_t rows, int64_t cols, int64_t ld, bool e5m2,
+                              const unsigned int* amax_bits, void* q, void* qt, float* scale_inv, cudaStream_t stream);
+// C[M,N] = A[M,K] * B[N,K]^T with both operands K-major fp8 (A E4M3, or E5M2 when a_e5m2; B E4M3), dequantized by the
+// device scalars 1/s_a, 1/s_b.  K % 16, lda % 16, ldb % 16 == 0 and 16-byte-aligned bases (TMA), N % 8 == 0.
+bool gemm_fp8_tn_supported(int64_t M, int64_t N, int64_t K, const void* A, const void* B, const void* C, int64_t lda,
+                           int64_t ldb, int64_t ldc);
+// C = bf16(gscale * acc / (s_a s_b)) (gscale optional)
+void launch_gemm_fp8_tn(const void* A, bool a_e5m2, const void* B, void* C, int64_t M, int64_t N, int64_t K, int64_t lda,
+                        int64_t ldb, int64_t ldc, const float* a_scale_inv, const float* b_scale_inv, const float* gscale,
+                        int sm_count, cudaStream_t stream);
+// A E4M3: dy = bf16(grad_scale (acc / (s_a s_b) - target)), the loss as MseEpilogue, *dy_amax = bits of max |dy|
+// over the stored bf16 values (atomicMax; zeroed by the caller).
+void launch_gemm_fp8_mse(const void* A, const void* B, void* dy, int64_t M, int64_t N, int64_t K, int64_t lda,
+                         int64_t ldb, int64_t ldc, const float* a_scale_inv, const float* b_scale_inv,
+                         const MseEpilogue& mse, unsigned int* dy_amax, int sm_count, cudaStream_t stream);
+// W[M,N] (bf16, in place) = bf16(W + alpha * gscale * acc / (s_a s_b)).
+void launch_gemm_fp8_sgd(const void* A, bool a_e5m2, const void* B, void* W, int64_t M, int64_t N, int64_t K,
+                         int64_t lda, int64_t ldb, int64_t ldw, const float* a_scale_inv, const float* b_scale_inv,
+                         float alpha, const float* gscale, int sm_count, cudaStream_t stream);
+
 // Plain device copy into the heap (used to stage the weight for the fused kernel).
 void launch_copy_bytes(void* dst, const void* src, int64_t bytes, int sm_count, cudaStream_t stream);
 

@@ -49,4 +49,17 @@ inline CUtensorMap make_tmap_bf16_sw128(const void* base, int64_t rows, int64_t 
   return m;
 }
 
+// Row-major [rows, cols] one-byte (fp8) matrix with leading dimension `ld` (bytes, a multiple of 16); boxes of
+// 128 contiguous bytes (one 128-byte swizzle span) x box_rows rows.
+inline CUtensorMap make_tmap_u8_sw128(const void* base, int64_t rows, int64_t cols, int64_t ld, int box_rows) {
+  CUtensorMap m;
+  const cuuint64_t dims[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
+  const cuuint64_t strides[1] = {static_cast<cuuint64_t>(ld)};
+  const cuuint32_t box[2] = {128u, static_cast<cuuint32_t>(box_rows)};
+  CUresult r = encode_tiled_2d(&m, CU_TENSOR_MAP_DATA_TYPE_UINT8, const_cast<void*>(base), dims, strides, box,
+                               CU_TENSOR_MAP_SWIZZLE_128B);
+  M4T_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed with code " << static_cast<int>(r));
+  return m;
+}
+
 }  // namespace m4t

@@ -118,6 +118,40 @@ __device__ __forceinline__ void mma_tile(float (&acc)[BN / 2], uint8_t* smem, Pi
   if (prev >= 0 && lane == 0) tc::mbar_arrive(&p->empty[prev]);
 }
 
+// fp8 sibling of mma_tile for 128 x 128 tiles with both operands K-major.  A 128-byte stage row holds 128 fp8
+// values, so one stage is a k-block of 128 and each of its four k32 steps advances the descriptors by 32 bytes,
+// exactly as the bf16 k16 steps do: the ring, the swizzle and the producer are the bf16 ones.
+// Split accumulation: each k-block is summed by the tensor core into `blk` (a fresh accumulator) and then added
+// into `acc` in fp32, so the tensor core's fp8 accumulation never spans more than 128 products.  The block must
+// have retired before it is added, so no k-block stays queued behind the adds.
+template <bool A_E5M2>
+__device__ __forceinline__ void mma_tile_fp8(float (&acc)[64], uint8_t* smem, Pipe* p, int& stage, uint32_t& phase,
+                                             int k_blocks, int wgi) {
+  const int lane = threadIdx.x & 31;
+  float blk[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+  for (int kb = 0; kb < k_blocks; ++kb) {
+    tc::mbar_wait(&p->full[stage], phase);
+    const uint32_t sa = tc::smem_u32(smem + stage * Tile<128>::kStageBytes);
+    const uint32_t sb = sa + kABytes;
+    const uint32_t a0 = sa + static_cast<uint32_t>(wgi) * (64 * 128);
+    tc::fence_regs(blk);
+    tc::wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      tc::wgmma_m64n128k32_fp8<A_E5M2>(blk, tc::make_desc_sw128(a0 + k * 32, 16), tc::make_desc_sw128(sb + k * 32, 16),
+                                       k ? 1u : 0u);
+    tc::wgmma_commit();
+    tc::wgmma_wait<0>();
+    tc::fence_regs(blk);
+    if (lane == 0) tc::mbar_arrive(&p->empty[stage]);
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] += blk[i];
+    advance<128>(stage, phase);
+  }
+}
+
 // Accumulator fragment of wgmma m64nN (fp32): thread (warp w of the warpgroup, lane l) holds, for
 // j = 0 .. N/8 - 1, columns 8j + 2(l % 4) + {0, 1} of rows 16w + l / 4 (acc[4j], acc[4j+1]) and
 // 16w + l / 4 + 8 (acc[4j+2], acc[4j+3]).

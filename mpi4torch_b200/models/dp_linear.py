@@ -15,6 +15,11 @@ With ``sgd_in_backward=False`` the weight gets an ordinary ``.grad`` and ``train
 ``train_step(x, t, micro_batches=K)`` with K > 1 accumulates the gradients of K equal chunks of the batch in
 ``model.accumulator`` (an :class:`AccumulatedSGD`, fp32 buffers, no parameter-sized collective in backward) and
 then updates once.
+
+``fp8=True`` runs both GEMMs of the step in fp8 (``dp_linear_mse(..., fp8=True)``, DESIGN §4.4): E4M3 ``x`` and weight
+average, E5M2 ``dy``, per-tensor power-of-two scales kept on the device.  The in-backward optimizer then updates the
+weight in the fp8 wgrad kernel's epilogue at one rank and through ``allreduce_axpy_`` at several.  Micro-batch
+accumulation is not available with fp8.
 """
 from __future__ import annotations
 
@@ -24,12 +29,14 @@ import mpi4torch_b200 as m4t
 from mpi4torch_b200.models.dp_mlp import accumulated_step
 from mpi4torch_b200.ops import (AccumulatedSGD, InBackwardSGD, allreduce_linear, dp_linear_mse,
                                 in_backward_sgd_supported)
+from mpi4torch_b200.ops.fp8 import dp_linear_mse_fp8_supported
 
 
 class DPLinearModel:
     def __init__(self, in_features: int = 4096, out_features: int = 4096, comm=None, device="cuda",
                  dtype=torch.bfloat16, lr: float = 1e-4, seed: int = 0, fused: bool = True,
-                 sgd_in_backward: bool = True, prefetch: bool = True, assume_replicated: bool = False):
+                 sgd_in_backward: bool = True, prefetch: bool = True, assume_replicated: bool = False,
+                 fp8: bool = False):
         self.comm = m4t.COMM_WORLD if comm is None else comm
         g = torch.Generator().manual_seed(seed)  # identical initial weights on every rank
         w = torch.randn(out_features, in_features, generator=g) * (in_features ** -0.5)
@@ -49,6 +56,7 @@ class DPLinearModel:
         self.sgd_in_backward = sgd_in_backward  # fused wgrad -> reduce-scatter -> SGD -> multicast in backward
         self.optimizer = InBackwardSGD(lr, prefetch=prefetch, assume_replicated=assume_replicated)
         self.accumulator = AccumulatedSGD(lr)  # train_step(..., micro_batches > 1)
+        self.fp8 = bool(fp8)
         self._opt_ok = {}
 
     # ------------------------------------------------------------------ graph construction
@@ -61,8 +69,13 @@ class DPLinearModel:
         key = (x.device, x.dtype, tuple(x.shape), tuple(x.stride()))
         ok = self._opt_ok.get(key)
         if ok is None:
-            ok = (x.dim() == 2 and x.dtype == torch.bfloat16 and self.weight.dtype == torch.bfloat16
-                  and in_backward_sgd_supported(x, self.weight, self.comm))
+            if self.fp8:
+                # the fp8 in-backward update runs wherever the fp8 kernels do
+                t_like = x.new_empty((x.shape[0], self.weight.shape[0])) if x.dim() == 2 else x
+                ok = dp_linear_mse_fp8_supported(x, self.weight, t_like, self.comm)
+            else:
+                ok = (x.dim() == 2 and x.dtype == torch.bfloat16 and self.weight.dtype == torch.bfloat16
+                      and in_backward_sgd_supported(x, self.weight, self.comm))
             self._opt_ok[key] = ok
         return ok
 
@@ -70,7 +83,7 @@ class DPLinearModel:
         """Global mean-squared-error loss as a differentiable one-element tensor."""
         opt = self.optimizer if self._in_backward(x) else None
         local = dp_linear_mse(x, self.weight, target, self.comm, loss_scale=1.0 / (x.shape[0] * self.comm.size),
-                              optimizer=opt, allow_fused=self.fused)
+                              optimizer=opt, allow_fused=self.fused, fp8=self.fp8)
         return self.comm.Allreduce(local, m4t.MPI_SUM)
 
     def _local_loss(self, x, target, loss_scale, accumulator):
@@ -83,6 +96,8 @@ class DPLinearModel:
         ``micro_batches`` = K > 1: K forwards and backwards over equal chunks of this rank's batch (K must divide it)
         into ``self.accumulator``, then one update; the loss returned is the whole batch's."""
         if micro_batches != 1:
+            if self.fp8:
+                raise ValueError("mpi4torch_b200: train_step(micro_batches > 1) is not available with fp8=True")
             return accumulated_step(self.comm, self.accumulator, self._local_loss, x, target, micro_batches)
         value = self.loss(x, target)
         value.backward()
@@ -107,6 +122,8 @@ class DPLinearModel:
         still takes a host-side step counter, so capture needs either ``fused=False`` or the
         prefetching in-backward optimizer (whose steady-state step contains no fused forward).
         """
+        if self.fp8 and self.comm.size > 1:
+            raise RuntimeError("graph capture of the fp8 step is available at one rank")
         prefetching = self._in_backward(x) and self.optimizer.prefetch and self.comm.size > 1
         if self.comm.size > 1 and self.fused and not prefetching:
             raise RuntimeError("graph capture needs fused=False or the prefetching in-backward optimizer "

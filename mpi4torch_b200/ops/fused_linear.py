@@ -28,6 +28,7 @@ import torch
 import torch.nn.functional as F
 
 import mpi4torch_b200 as m4t
+from mpi4torch_b200.ops.fp8 import dp_linear_mse_fp8
 
 
 def has_fused_kernel() -> bool:
@@ -362,17 +363,23 @@ def in_backward_sgd_supported(x: torch.Tensor, weight: torch.Tensor, comm) -> bo
 
 def dp_linear_mse(x: torch.Tensor, weight: torch.Tensor, target: torch.Tensor, comm=None, *, loss_scale: float,
                   optimizer: Optional[InBackwardSGD] = None, allow_fused: bool = True,
-                  accumulator: Optional[AccumulatedSGD] = None) -> torch.Tensor:
+                  accumulator: Optional[AccumulatedSGD] = None, fp8: bool = False) -> torch.Tensor:
     """``loss_scale * sum((x @ mean_ranks(weight)^T - target)^2)`` of THIS rank's batch as a
     differentiable one-element fp32 tensor; sum it over ranks with ``comm.Allreduce``.
 
     ``optimizer``: an :class:`InBackwardSGD` makes ``backward`` apply the SGD step itself (fused
     into the gradient reduce-scatter); the weight then receives no ``.grad``.
     ``accumulator``: an :class:`AccumulatedSGD` makes ``backward`` add this rank's gradient into its buffer
-    (no collective, no ``.grad``); ``accumulator.step()`` updates the weight.  Not combinable with ``optimizer``."""
+    (no collective, no ``.grad``); ``accumulator.step()`` updates the weight.  Not combinable with ``optimizer``.
+    ``fp8``: run both GEMMs in fp8 with per-tensor power-of-two scaling (:mod:`mpi4torch_b200.ops.fp8`); ``x.grad``
+    stays the bf16 dgrad.  Not combinable with ``accumulator``."""
     c = m4t.COMM_WORLD if comm is None else comm
     if accumulator is not None and optimizer is not None:
         raise ValueError("mpi4torch_b200: dp_linear_mse takes either optimizer= or accumulator=, not both")
+    if fp8:
+        if accumulator is not None:
+            raise ValueError("mpi4torch_b200: dp_linear_mse(fp8=True) does not support accumulator=")
+        return dp_linear_mse_fp8(x, weight, target, c, loss_scale, optimizer)
     if accumulator is not None:
         if dp_linear_mse_supported(x, weight, target, c):
             return _DPLinearMSEAccumulate.apply(x, weight, target, [c], float(loss_scale), accumulator,
