@@ -1,0 +1,130 @@
+"""Forward + backward of the experts of a mixture-of-experts layer (``expert_mlp``) at one rank, three arms:
+
+* ``batched``: the ``expert_mlp`` node, one launch per GEMM for all E experts;
+* ``loop``: the same math with the same bits as a loop over experts of the single-expert ops
+  (``linear_bias_gelu_forward``, whose ``z`` output stands in for the bias-only layer, ``gemm_nn_gelu_backward``,
+  ``wgrad_bf16``, ``gemm_bf16_nn``, ``column_sum``);
+* ``eager``: bf16 ``baddbmm`` / ``F.gelu`` / autograd.
+
+Two shapes: E = 8, M = 256, D = 1024, H = 4096, where one expert's GEMM is a fraction of a wave, and E = 8,
+M = 1024, D = 4096, H = 16384, where it is several waves.  Step times come from CUDA events over windows of
+``--steps`` calls, the arms alternated, ``--reps`` windows each (min / median / max reported); per-kernel times from
+a separate ``torch.profiler`` run; FLOP/s from the shapes (forward 2 E M (D H + H O), backward twice that).  The card
+name and power limit are read in the same run.
+
+    python benchmarks/moe_step.py [--shapes small,large] [--out DIR]
+"""
+import argparse
+import json
+import os
+import statistics
+import sys
+
+import torch
+import torch.nn.functional as F
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+import mpi4torch_b200 as m4t  # noqa: E402
+from benchmarks.fp8_linear_step import kernel_times  # noqa: E402
+from benchmarks.mlp_step import card, time_ms  # noqa: E402
+from mpi4torch_b200.ops import expert_mlp, expert_mlp_supported  # noqa: E402
+
+SHAPES = {"small": (8, 256, 1024, 4096), "large": (8, 1024, 4096, 16384)}  # E, M, D, H (O = D)
+
+
+def short(name):
+    """A kernel's name with its template arguments (the last one of the GEMMs and the column sum is BATCHED)."""
+    return name.split("(CU")[0].split("(float")[0].replace("void ", "").replace("m4t::", "").replace(
+        "(anonymous namespace)::", "")[:80]
+
+
+def make_arms(E, M, D, H):
+    g = torch.Generator(device="cuda").manual_seed(0)
+    r = lambda *s, scale=1.0: (torch.randn(*s, generator=g, device="cuda") * scale)  # noqa: E731
+    x = r(E, M, D).to(torch.bfloat16)
+    w1, w2 = r(E, H, D, scale=D ** -0.5).to(torch.bfloat16), r(E, D, H, scale=H ** -0.5).to(torch.bfloat16)
+    b1, b2 = r(E, H, scale=0.1), r(E, D, scale=0.1)
+    dy = r(E, M, D).to(torch.bfloat16)
+    params = [t.requires_grad_() for t in (x, w1, b1, w2, b2)]
+    assert expert_mlp_supported(*params)
+    ops = torch.ops.mpi4torch_b200
+
+    def batched():
+        y = expert_mlp(*params)
+        y.backward(dy)
+
+    def loop():
+        for e in range(E):
+            xe, w1e, w2e = x.detach()[e], w1.detach()[e], w2.detach()[e]
+            h, z = ops.linear_bias_gelu_forward(xe, w1e, b1.detach()[e])
+            ops.linear_bias_gelu_forward(h, w2e, b2.detach()[e])
+            dz, part = ops.gemm_nn_gelu_backward(dy[e], w2e, z)
+            ops.wgrad_bf16(dy[e], h)
+            ops.gemm_bf16_nn(dz, w1e)
+            ops.wgrad_bf16(dz, xe)
+            ops.column_sum(part)
+        dy.sum(1, dtype=torch.float32)
+
+    bf = [t.detach().to(torch.bfloat16).requires_grad_() for t in params]
+
+    def eager():
+        xe, w1e, b1e, w2e, b2e = bf
+        h = F.gelu(torch.baddbmm(b1e.unsqueeze(1), xe, w1e.transpose(1, 2)), approximate="tanh")
+        y = torch.baddbmm(b2e.unsqueeze(1), h, w2e.transpose(1, 2))
+        y.backward(dy)
+
+    def clear():
+        for t in params + bf:
+            t.grad = None
+
+    return {"batched": batched, "loop": loop, "eager": eager}, clear
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--shapes", default="small,large")
+    ap.add_argument("--steps", type=int, default=50)
+    ap.add_argument("--warmup", type=int, default=20)
+    ap.add_argument("--reps", type=int, default=6)
+    ap.add_argument("--out", default=None, help="directory for the profiler traces")
+    a = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("moe_step.py measures on the GPU; none is visible")
+    assert m4t.COMM_WORLD.size == 1 and m4t.cuda_backend_ready()
+    if a.out:
+        os.makedirs(a.out, exist_ok=True)
+    for tag in a.shapes.split(","):
+        E, M, D, H = SHAPES[tag]
+        arms, clear = make_arms(E, M, D, H)
+        res = {"card": card(), "shape": {"E": E, "M": M, "D": D, "H": H, "O": D}}
+        for fn in arms.values():
+            for _ in range(a.warmup):
+                fn()
+                clear()
+        torch.cuda.synchronize()
+        times = {k: [] for k in arms}
+        names = list(arms)
+        for rep in range(a.reps):
+            order = names if rep % 2 == 0 else names[::-1]
+            for k in order:
+                times[k].append(time_ms(lambda k=k: (arms[k](), clear()), a.steps))
+        flops = 3 * 2.0 * E * M * (D * H + H * D)
+        res["step_ms"] = {k: {"min": round(min(v), 4), "median": round(statistics.median(v), 4), "max": round(max(v), 4),
+                              "tflops_at_median": round(flops / (statistics.median(v) * 1e-3) / 1e12, 1)}
+                          for k, v in times.items()}
+        for k in ("batched", "loop"):
+            kt = kernel_times(lambda k=k: (arms[k](), clear()), 10, None, k)
+            merged = {}
+            for name, ms in kt.items():
+                merged[short(name)] = merged.get(short(name), 0.0) + ms
+            total = sum(merged.values())
+            res[f"kernels_ms_{k}"] = {n: round(v, 4) for n, v in sorted(merged.items(), key=lambda kv: -kv[1])}
+            res[f"device_ms_{k}"] = round(total, 4)
+            res[f"device_tflops_{k}"] = round(flops / (total * 1e-3) / 1e12, 1)
+        res["launches_per_step"] = {"batched": 7, "loop": 7 * E}
+        print(json.dumps(res), flush=True)
+
+
+if __name__ == "__main__":
+    main()

@@ -444,6 +444,134 @@ Tensor column_sum(const Tensor& partials, const c10::optional<Tensor>& grad_scal
   return out;
 }
 
+// ---- batched experts (E experts of one shape per launch) ---------------------------------------------------------
+// Operands are contiguous bf16 CUDA tensors stacked along dim 0 on one device; see batched_gemm_supported.
+bool bf16_3d(const Tensor& t) {
+  return t.is_cuda() && t.dim() == 3 && t.scalar_type() == at::kBFloat16 && t.is_contiguous();
+}
+
+bool same_device(std::initializer_list<const Tensor*> ts) {
+  for (const Tensor* t : ts)
+    if (t->device() != (*ts.begin())->device()) return false;
+  return true;
+}
+
+// x [E, M, K] @ w [E, N, K]^T, and the bias [E, N] (contiguous fp32, 8-byte aligned) when given.
+bool batched_gemm_tn_ok(const Tensor& x, const Tensor& w, const c10::optional<Tensor>& bias) {
+  if (!(bf16_3d(x) && bf16_3d(w) && same_device({&x, &w}) && x.size(0) == w.size(0) && x.size(2) == w.size(2)))
+    return false;
+  if (bias.has_value() && !(bias->is_cuda() && bias->device() == x.device() && bias->dim() == 2 &&
+                            bias->scalar_type() == at::kFloat && bias->is_contiguous() && bias->size(0) == w.size(0) &&
+                            bias->size(1) == w.size(1) && epilogue_bias_ok(bias->data_ptr<float>())))
+    return false;
+  return World::instance().cuda_ready() &&
+         batched_gemm_supported(x.size(0), x.size(1), w.size(1), x.size(2), x.data_ptr(), w.data_ptr(), x.data_ptr());
+}
+
+// a [E, M, K] @ b [E, K, N].
+bool batched_gemm_nn_ok(const Tensor& a, const Tensor& b) {
+  if (!(bf16_3d(a) && bf16_3d(b) && same_device({&a, &b}) && a.size(0) == b.size(0) && a.size(2) == b.size(1)))
+    return false;
+  return World::instance().cuda_ready() &&
+         batched_gemm_supported(a.size(0), a.size(1), b.size(2), a.size(2), a.data_ptr(), b.data_ptr(), a.data_ptr());
+}
+
+// dy [E, M, N]^T @ x [E, M, K] per expert.
+bool batched_wgrad_bf16_ok(const Tensor& dy, const Tensor& x) {
+  if (!(bf16_3d(dy) && bf16_3d(x) && same_device({&dy, &x}) && dy.size(0) == x.size(0) && dy.size(1) == x.size(1)))
+    return false;
+  return World::instance().cuda_ready() && wgrad_bf16_batched_supported(dy.size(0), dy.size(1), dy.size(2), x.size(2),
+                                                                         dy.data_ptr(), x.data_ptr(), x.data_ptr());
+}
+
+cudaStream_t stream_of(const Tensor& t) { return c10::cuda::getCurrentCUDAStream(t.device().index()).stream(); }
+
+int sm_count() { return backend().device_comm().sm_count; }
+
+// (h, z) per expert: z_e = x_e @ w_e^T + b_e, h_e = gelu_tanh(z_e), as linear_bias_gelu_forward, in one launch.
+std::tuple<Tensor, Tensor> batched_linear_bias_gelu_forward(const Tensor& x, const Tensor& w, const Tensor& b) {
+  TORCH_CHECK(batched_gemm_tn_ok(x, w, b),
+              "mpi4torch_b200: batched_linear_bias_gelu_forward needs contiguous bf16 x [E, M, K], w [E, N, K] and fp32 "
+              "b [E, N] on one CUDA device, M % 128 == N % 128 == K % 128 == 0, and aligned bases");
+  c10::cuda::CUDAGuard guard(x.device());
+  Tensor z = at::empty({x.size(0), x.size(1), w.size(1)}, x.options());
+  Tensor h = at::empty_like(z);
+  std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
+  launch_gemm_bias_gelu_batched(x.data_ptr(), w.data_ptr(), b.data_ptr<float>(), z.data_ptr(), h.data_ptr(), x.size(0),
+                                x.size(1), w.size(1), x.size(2), sm_count(), stream_of(x));
+  return {h, z};
+}
+
+// y_e = bf16(x_e @ w_e^T + b_e), one launch.
+Tensor batched_linear_bias_forward(const Tensor& x, const Tensor& w, const Tensor& b) {
+  TORCH_CHECK(batched_gemm_tn_ok(x, w, b),
+              "mpi4torch_b200: batched_linear_bias_forward needs contiguous bf16 x [E, M, K], w [E, N, K] and fp32 "
+              "b [E, N] on one CUDA device, M % 128 == N % 128 == K % 128 == 0, and aligned bases");
+  c10::cuda::CUDAGuard guard(x.device());
+  Tensor y = at::empty({x.size(0), x.size(1), w.size(1)}, x.options());
+  std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
+  launch_gemm_bias_batched(x.data_ptr(), w.data_ptr(), b.data_ptr<float>(), y.data_ptr(), x.size(0), x.size(1), w.size(1),
+                           x.size(2), sm_count(), stream_of(x));
+  return y;
+}
+
+// (dz, partials) per expert: dz_e = grad_scale * (dy_e @ w_e) * gelu_tanh'(z_e) (w [E, K, N] read in place), and the
+// column-sum partials of dz as [E, M / 16, N] (reduce them with batched_column_sum).
+std::tuple<Tensor, Tensor> batched_gemm_nn_gelu_backward(const Tensor& dy, const Tensor& w, const Tensor& z,
+                                                         const c10::optional<Tensor>& grad_scale) {
+  TORCH_CHECK(batched_gemm_nn_ok(dy, w) && bf16_3d(z) && z.device() == dy.device() && z.size(0) == dy.size(0) &&
+                  z.size(1) == dy.size(1) && z.size(2) == w.size(2),
+              "mpi4torch_b200: batched_gemm_nn_gelu_backward needs contiguous bf16 dy [E, M, K], w [E, K, N] and "
+              "z [E, M, N] on one CUDA device, M % 128 == N % 128 == K % 128 == 0, and aligned bases");
+  c10::cuda::CUDAGuard guard(dy.device());
+  const int64_t E = dy.size(0), M = dy.size(1), N = w.size(2);
+  Tensor dz = at::empty({E, M, N}, dy.options());
+  Tensor part = at::empty({E, colsum_rows(M), N}, dy.options().dtype(at::kFloat));
+  std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
+  launch_gemm_nn_gelu_bwd_colsum_batched(dy.data_ptr(), w.data_ptr(), z.data_ptr(), dz.data_ptr(), part.data_ptr<float>(),
+                                         E, M, N, dy.size(2), sm_count(), stream_of(dy), grad_scale_ptr(grad_scale, dy));
+  return {dz, part};
+}
+
+// c_e = a_e @ b_e with b [E, K, N] read in place, one launch.
+Tensor batched_gemm_nn(const Tensor& a, const Tensor& b) {
+  TORCH_CHECK(batched_gemm_nn_ok(a, b),
+              "mpi4torch_b200: batched_gemm_nn needs contiguous bf16 a [E, M, K] and b [E, K, N] on one CUDA device, "
+              "M % 128 == N % 128 == K % 128 == 0, and 16-byte-aligned bases");
+  c10::cuda::CUDAGuard guard(a.device());
+  Tensor c = at::empty({a.size(0), a.size(1), b.size(2)}, a.options());
+  std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
+  launch_gemm_nn_batched(a.data_ptr(), b.data_ptr(), c.data_ptr(), a.size(0), a.size(1), b.size(2), a.size(2), sm_count(),
+                         stream_of(a));
+  return c;
+}
+
+// G_e = grad_scale * dy_e^T @ x_e -> [E, N, K], one launch.
+Tensor batched_wgrad_bf16(const Tensor& dy, const Tensor& x, const c10::optional<Tensor>& grad_scale) {
+  TORCH_CHECK(batched_wgrad_bf16_ok(dy, x),
+              "mpi4torch_b200: batched_wgrad_bf16 needs contiguous bf16 dy [E, M, N] and x [E, M, K] on one CUDA device, "
+              "N % 128 == K % 128 == M % 64 == 0, and 16-byte-aligned bases");
+  c10::cuda::CUDAGuard guard(x.device());
+  Tensor gw = at::empty({dy.size(0), dy.size(2), x.size(2)}, x.options());
+  std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
+  launch_wgrad_bf16_batched(dy.data_ptr(), x.data_ptr(), gw.data_ptr(), dy.size(0), dy.size(1), dy.size(2), x.size(2),
+                            sm_count(), stream_of(x), grad_scale_ptr(grad_scale, x));
+  return gw;
+}
+
+// out[e, n] = grad_scale * sum_i partials[e, i, n] (fp32), in column_sum's fixed order, one launch.
+Tensor batched_column_sum(const Tensor& partials, const c10::optional<Tensor>& grad_scale) {
+  TORCH_CHECK(partials.is_cuda() && partials.dim() == 3 && partials.scalar_type() == at::kFloat &&
+                  partials.is_contiguous() && partials.size(0) > 0 && partials.size(1) > 0,
+              "mpi4torch_b200: batched_column_sum needs a non-empty contiguous 3-d fp32 CUDA tensor");
+  c10::cuda::CUDAGuard guard(partials.device());
+  Tensor out = at::empty({partials.size(0), partials.size(2)}, partials.options());
+  if (out.numel() == 0) return out;
+  launch_column_sum_batched(partials.data_ptr<float>(), partials.size(0), partials.size(1), partials.size(2),
+                            out.data_ptr<float>(), grad_scale_ptr(grad_scale, partials), stream_of(partials));
+  return out;
+}
+
 // ---- FP8 linear layer (gemm_fp8.cu) ------------------------------------------------------------------------------
 bool fp8_e5m2(c10::string_view fmt) {
   TORCH_CHECK(fmt == "e4m3" || fmt == "e5m2", "mpi4torch_b200: the fp8 format must be 'e4m3' or 'e5m2'");
@@ -588,6 +716,17 @@ TORCH_LIBRARY_FRAGMENT(mpi4torch_b200, m) {
   m.def("gemm_fp8_tn_sgd_(Tensor(a!) w, Tensor a, Tensor b, Tensor a_scale_inv, Tensor b_scale_inv, float scale, "
         "Tensor? grad_scale=None) -> ()",
         &gemm_fp8_tn_sgd_);
+  m.def("batched_gemm_tn_supported(Tensor x, Tensor w, Tensor? bias=None) -> bool", &batched_gemm_tn_ok);
+  m.def("batched_gemm_nn_supported(Tensor a, Tensor b) -> bool", &batched_gemm_nn_ok);
+  m.def("batched_wgrad_bf16_supported(Tensor dy, Tensor x) -> bool", &batched_wgrad_bf16_ok);
+  m.def("batched_linear_bias_gelu_forward(Tensor x, Tensor w, Tensor b) -> (Tensor, Tensor)",
+        &batched_linear_bias_gelu_forward);
+  m.def("batched_linear_bias_forward(Tensor x, Tensor w, Tensor b) -> Tensor", &batched_linear_bias_forward);
+  m.def("batched_gemm_nn_gelu_backward(Tensor dy, Tensor w, Tensor z, Tensor? grad_scale=None) -> (Tensor, Tensor)",
+        &batched_gemm_nn_gelu_backward);
+  m.def("batched_gemm_nn(Tensor a, Tensor b) -> Tensor", &batched_gemm_nn);
+  m.def("batched_wgrad_bf16(Tensor dy, Tensor x, Tensor? grad_scale=None) -> Tensor", &batched_wgrad_bf16);
+  m.def("batched_column_sum(Tensor partials, Tensor? grad_scale=None) -> Tensor", &batched_column_sum);
   m.def("linear_bias_gelu_forward(Tensor x, Tensor w, Tensor b) -> (Tensor, Tensor)", &linear_bias_gelu_forward);
   m.def("linear_bias_mse_forward_local(Tensor x, Tensor w, Tensor b, Tensor target, float loss_scale, float grad_scale) "
         "-> (Tensor, Tensor, Tensor)",

@@ -42,6 +42,9 @@ struct GemmArgs {
   // fused mode ----------------------------------------------------------------
   const uint32_t* panel_flags;  // [N / kPanel] counters in local HBM (written through multicast)
   uint32_t panel_target;        // a panel is ready when its counter >= target (wrap-safe)
+  // batched kernels: rows of one expert (a multiple of BM).  Placed in the tail padding, so the other
+  // kernels' parameter layout is unchanged.
+  int expert_rows;
 };
 
 // the fused kernel's communication warps need registers: half-width tiles there
@@ -52,6 +55,7 @@ template <bool FUSED> constexpr int tile_n() { return FUSED ? 128 : 256; }
 //   EPI 3  TN  d = acc + bias - T:  C = grad_scale * d, loss as EPI 1, column-sum partials of C
 //   EPI 4  NN  C = gscale * acc * gelu_tanh'(z), z read from T (bf16), column-sum partials of C
 //   EPI 5  TN  C = logits = acc + bias, per-tile softmax partials (xent_epilogue; xent_finish completes them)
+//   EPI 6  TN  C = acc + bias (EPI 2 without h)
 // Column sums are deterministic: a warp adds its 16 rows in registers (h pair, then lane bits 2-4) and
 // lanes 0-3 store one fp32 row of colsum[ceil(M/16), N]; column_sum_kernel adds those rows in a fixed order.
 struct MlpEpiArgs {
@@ -83,7 +87,7 @@ template <int EPI, int BN>
 __device__ __forceinline__ void mlp_epilogue(const float (&acc)[BN / 2], const GemmArgs& g, const MlpEpiArgs& e,
                                              int m_blk, int n_blk, int wgi, float& loss_part) {
   constexpr int kGroup = 4;
-  constexpr bool kBias = EPI != 4, kReadT = EPI != 2, kColsum = EPI != 2;
+  constexpr bool kBias = EPI != 4, kReadT = EPI == 3 || EPI == 4, kColsum = EPI == 3 || EPI == 4;
   const int lane = threadIdx.x & 31;
   const int row0 = m_blk * BM + wgi * 64 + frag_row(0);
   const bool row_ok[2] = {row0 < g.M, row0 + 8 < g.M};
@@ -133,7 +137,7 @@ __device__ __forceinline__ void mlp_epilogue(const float (&acc)[BN / 2], const G
           loss_part = fmaf(d1, d1, loss_part);
           v0 = d0 * g.grad_scale;
           v1 = d1 * g.grad_scale;
-        } else {
+        } else if (EPI == 4) {
           v0 = gs * v0 * gelu_tanh_grad(t0);
           v1 = gs * v1 * gelu_tanh_grad(t1);
         }
@@ -215,7 +219,9 @@ __device__ __forceinline__ void xent_epilogue(float (&acc)[BN / 2], const GemmAr
   }
 }
 
-template <bool FUSED, int EPI, bool B_MN>
+// BATCHED: E experts stacked along M (g.M = E * g.expert_rows); the tile's expert is m0 / expert_rows.  Only B and
+// the bias depend on it: B is one map over the stacked weights, read at row offset expert * (N, or K if B_MN).
+template <bool FUSED, int EPI, bool B_MN, bool BATCHED = false>
 __global__ void __launch_bounds__(kGemmThreads + (FUSED ? kCommWarps * 32 : 0), 1)
 gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                        const GemmArgs g, const CommArgs cm, const MlpEpiArgs e) {
@@ -257,8 +263,10 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
           bounded_wait_ge(g.panel_flags + n_blk * BN / kPanel, g.panel_target, cm.sync);
           tc::fence_proxy_async();  // generic-proxy writes (multimem.st) -> async-proxy reads (TMA)
         }
+        const int b_row0 = BATCHED ? (m_blk * BM / g.expert_rows) * (B_MN ? g.K : g.N) : 0;
         for (int kb = 0; kb < k_blocks; ++kb)
-          load_stage<false, B_MN, BN>(smem, pipe, stage, phase, &tmap_a, &tmap_b, m_blk * BM, n_blk * BN, kb * BK);
+          load_stage<false, B_MN, BN>(smem, pipe, stage, phase, &tmap_a, &tmap_b, m_blk * BM, n_blk * BN, kb * BK,
+                                      b_row0);
       }
     }
   } else if (warp < kGemmThreads / 32) {
@@ -275,6 +283,10 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
       float loss_part = 0.f;
       if constexpr (EPI == 5) {
         xent_epilogue<BN>(acc, g, e, m_blk, n_blk, wgi);
+      } else if constexpr (EPI >= 2 && BATCHED) {
+        MlpEpiArgs ex = e;
+        if (e.bias != nullptr) ex.bias = e.bias + static_cast<int64_t>(m_blk * BM / g.expert_rows) * g.N;
+        mlp_epilogue<EPI, BN>(acc, g, ex, m_blk, n_blk, wgi, loss_part);
       } else if constexpr (EPI >= 2) {
         mlp_epilogue<EPI, BN>(acc, g, e, m_blk, n_blk, wgi, loss_part);
       } else {
@@ -336,20 +348,20 @@ CUtensorMap make_tmap(const void* base, int64_t rows, int64_t cols, int64_t ld, 
 
 template <bool FUSED> constexpr int smem_bytes() { return Tile<tile_n<FUSED>()>::kSmemBytes; }
 
-template <bool FUSED, int EPI, bool B_MN> void configure_once() {
+template <bool FUSED, int EPI, bool B_MN, bool BATCHED> void configure_once() {
   static std::once_flag once;
   std::call_once(once, [] {
-    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<FUSED, EPI, B_MN>,
+    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<FUSED, EPI, B_MN, BATCHED>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes<FUSED>());
     M4T_CHECK(e == cudaSuccess, "cudaFuncSetAttribute(smem) failed: " << cudaGetErrorString(e));
   });
 }
 
-template <bool FUSED, int EPI, bool B_MN>
+template <bool FUSED, int EPI, bool B_MN, bool BATCHED = false>
 void launch(int grid, const CUtensorMap& ta, const CUtensorMap& tb, const GemmArgs& g, const CommArgs& cm,
             cudaStream_t stream, const char* what, const MlpEpiArgs& e = MlpEpiArgs{}) {
-  configure_once<FUSED, EPI, B_MN>();
-  gemm_bf16_wgmma_kernel<FUSED, EPI, B_MN>
+  configure_once<FUSED, EPI, B_MN, BATCHED>();
+  gemm_bf16_wgmma_kernel<FUSED, EPI, B_MN, BATCHED>
       <<<grid, kGemmThreads + (FUSED ? kCommWarps * 32 : 0), smem_bytes<FUSED>(), stream>>>(ta, tb, g, cm, e);
   cudaError_t err = cudaGetLastError();
   M4T_CHECK(err == cudaSuccess, what << " launch failed: " << cudaGetErrorString(err));
@@ -366,9 +378,15 @@ void set_mse(GemmArgs& g, const MseEpilogue* mse) {
 
 // out[n] = gscale * sum_i partial[i, n] over i = 0, 1, .. in a fixed order: a block covers 32 columns,
 // its 8 row groups each add every 8th row, and row group 0 adds the 8 results in order.
+// BATCHED: expert e = blockIdx.y reduces partial[e] [rows, N] into out[e] [N] in that same order.
+template <bool BATCHED = false>
 __global__ void __launch_bounds__(256) column_sum_kernel(const float* __restrict__ partial, int rows, int N,
                                                          float* __restrict__ out, const float* gscale) {
   __shared__ float part[8][33];
+  if (BATCHED) {
+    partial += static_cast<int64_t>(blockIdx.y) * rows * N;
+    out += static_cast<int64_t>(blockIdx.y) * N;
+  }
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
   const int n = blockIdx.x * 32 + tx;
   float s = 0.f;
@@ -716,5 +734,83 @@ void launch_xent_finish(void* y, int64_t M, int64_t N, int64_t ldy, const float2
 }
 
 int fused_gemm_grid(const DeviceComm& dc) { return std::min(dc.sm_count, kMaxChannels) & ~1; }
+
+// ---- batched experts ---------------------------------------------------------------------------------------------
+// Every operand is contiguous and stacked along its leading dimension, so expert e's A rows are rows [e M, e M + M) of
+// one [E M, K] matrix and the whole call is ONE GEMM of E M rows against a B that changes at every M rows.
+bool batched_gemm_supported(int64_t E, int64_t M, int64_t N, int64_t K, const void* A, const void* B, const void* C) {
+  auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
+  return E > 0 && M > 0 && N > 0 && K > 0 && M % BM == 0 && N % 128 == 0 && K % 128 == 0 && al16(A) && al16(B) &&
+         al16(C) && E * M < (1ll << 31) && E * N < (1ll << 31) && E * K < (1ll << 31);
+}
+
+namespace {
+
+GemmArgs batched_args(void* C, int64_t E, int64_t M, int64_t N, int64_t K) {
+  GemmArgs g = plain_args(C, E * M, N, K, N);
+  g.expert_rows = static_cast<int>(M);
+  return g;
+}
+
+}  // namespace
+
+void launch_gemm_bias_gelu_batched(const void* A, const void* B, const float* bias, void* z, void* h, int64_t E,
+                                   int64_t M, int64_t N, int64_t K, int sm_count, cudaStream_t stream) {
+  M4T_CHECK(batched_gemm_supported(E, M, N, K, A, B, z) && (reinterpret_cast<uintptr_t>(h) & 15u) == 0 &&
+                epilogue_bias_ok(bias),
+            "unsupported shape/alignment for the batched bias+GELU GEMM");
+  MlpEpiArgs e{};
+  e.bias = bias;
+  e.h_out = h;
+  launch<false, 2, false, true>(plain_grid(E * M, N, sm_count), make_tmap(A, E * M, K, K, BM),
+                                make_tmap(B, E * N, K, K, tile_n<false>()), batched_args(z, E, M, N, K), CommArgs{},
+                                stream, "gemm_bias_gelu_batched", e);
+}
+
+void launch_gemm_bias_batched(const void* A, const void* B, const float* bias, void* y, int64_t E, int64_t M, int64_t N,
+                              int64_t K, int sm_count, cudaStream_t stream) {
+  M4T_CHECK(batched_gemm_supported(E, M, N, K, A, B, y) && epilogue_bias_ok(bias),
+            "unsupported shape/alignment for the batched bias GEMM");
+  MlpEpiArgs e{};
+  e.bias = bias;
+  launch<false, 6, false, true>(plain_grid(E * M, N, sm_count), make_tmap(A, E * M, K, K, BM),
+                                make_tmap(B, E * N, K, K, tile_n<false>()), batched_args(y, E, M, N, K), CommArgs{},
+                                stream, "gemm_bias_batched", e);
+}
+
+void launch_gemm_nn_gelu_bwd_colsum_batched(const void* A, const void* B, const void* z, void* dz, float* colsum,
+                                            int64_t E, int64_t M, int64_t N, int64_t K, int sm_count, cudaStream_t stream,
+                                            const float* gscale) {
+  M4T_CHECK(batched_gemm_supported(E, M, N, K, A, B, dz) && epilogue_bf16_pairs_ok(z, N),
+            "unsupported shape/alignment for the batched GELU-backward GEMM");
+  GemmArgs g = batched_args(dz, E, M, N, K);
+  g.T = z;
+  g.ldt = static_cast<int>(N);
+  MlpEpiArgs e{};
+  e.colsum = colsum;
+  e.gscale = gscale;
+  launch<false, 4, true, true>(plain_grid(E * M, N, sm_count), make_tmap(A, E * M, K, K, BM),
+                               make_tmap_bf16_sw128(B, E * K, N, N, 64, BK), g, CommArgs{}, stream,
+                               "gemm_nn_gelu_bwd_colsum_batched", e);
+}
+
+void launch_gemm_nn_batched(const void* A, const void* B, void* C, int64_t E, int64_t M, int64_t N, int64_t K,
+                            int sm_count, cudaStream_t stream) {
+  M4T_CHECK(batched_gemm_supported(E, M, N, K, A, B, C), "unsupported shape/alignment for the batched NN GEMM");
+  launch<false, 0, true, true>(plain_grid(E * M, N, sm_count), make_tmap(A, E * M, K, K, BM),
+                               make_tmap_bf16_sw128(B, E * K, N, N, 64, BK), batched_args(C, E, M, N, K), CommArgs{},
+                               stream, "gemm_nn_batched");
+}
+
+void launch_column_sum_batched(const float* partial, int64_t E, int64_t rows, int64_t N, float* out, const float* gscale,
+                               cudaStream_t stream) {
+  M4T_CHECK(E > 0 && E < 65536 && rows > 0 && N > 0 && N < (1ll << 31) && rows * N < (1ll << 31),
+            "column_sum_batched: empty or oversized workspace");
+  const dim3 grid(static_cast<unsigned>((N + 31) / 32), static_cast<unsigned>(E));
+  column_sum_kernel<true><<<grid, 256, 0, stream>>>(partial, static_cast<int>(rows), static_cast<int>(N), out, gscale);
+  cudaError_t err = cudaGetLastError();
+  M4T_CHECK(err == cudaSuccess, "column_sum_batched launch failed: " << cudaGetErrorString(err));
+  note_kernel_launch("column_sum_batched");
+}
 
 }  // namespace m4t

@@ -201,6 +201,33 @@ void launch_fused_wgrad_update(const DeviceComm& dc, const void* dy, const void*
 // wavg_off >= 0: additionally leaves (1/P) * sum_ranks W_new in the bf16 [N,K] buffer at that heap
 // offset on every rank (the parameter all-reduce of the NEXT forward, run under this GEMM).
 
+// ---- batched experts (gemm_wgmma.cu, wgrad_wgmma.cu; DESIGN §4.4) -------------------------------------------------
+// E experts of identical shapes in ONE launch.  Every operand is contiguous and stacked along its leading dimension:
+// A [E, M, K], B [E, N, K] (TN) or [E, K, N] (NN), C [E, M, N], bias [E, N] fp32, column-sum partials
+// [E, M / 16, N].  M % 128 == 0 (a tile never spans two experts), N % 128 == K % 128 == 0, 16-byte-aligned bases.
+bool batched_gemm_supported(int64_t E, int64_t M, int64_t N, int64_t K, const void* A, const void* B, const void* C);
+// z_e = A_e B_e^T + bias_e, h_e = gelu_tanh(z_e), as launch_gemm_bias_gelu per expert.
+void launch_gemm_bias_gelu_batched(const void* A, const void* B, const float* bias, void* z, void* h, int64_t E,
+                                   int64_t M, int64_t N, int64_t K, int sm_count, cudaStream_t stream);
+// y_e = bf16(A_e B_e^T + bias_e).
+void launch_gemm_bias_batched(const void* A, const void* B, const float* bias, void* y, int64_t E, int64_t M, int64_t N,
+                              int64_t K, int sm_count, cudaStream_t stream);
+// dz_e = gscale * (A_e B_e) * gelu_tanh'(z_e) and its column-sum partials, as launch_gemm_nn_gelu_bwd_colsum.
+void launch_gemm_nn_gelu_bwd_colsum_batched(const void* A, const void* B, const void* z, void* dz, float* colsum,
+                                            int64_t E, int64_t M, int64_t N, int64_t K, int sm_count, cudaStream_t stream,
+                                            const float* gscale = nullptr);
+// C_e = A_e B_e, as launch_gemm_bf16_nn.
+void launch_gemm_nn_batched(const void* A, const void* B, void* C, int64_t E, int64_t M, int64_t N, int64_t K,
+                            int sm_count, cudaStream_t stream);
+// out[e, n] = gscale * sum_i partial[e, i, n], in column_sum's order.
+void launch_column_sum_batched(const float* partial, int64_t E, int64_t rows, int64_t N, float* out, const float* gscale,
+                               cudaStream_t stream);
+// G_e [N, K] = gscale * dY_e^T X_e with dY [E, Mb, N], X [E, Mb, K], G [E, N, K]; the rules of wgrad_bf16_supported.
+bool wgrad_bf16_batched_supported(int64_t E, int64_t Mb, int64_t N, int64_t K, const void* dy, const void* x,
+                                  const void* g);
+void launch_wgrad_bf16_batched(const void* dy, const void* x, void* g, int64_t E, int64_t Mb, int64_t N, int64_t K,
+                               int sm_count, cudaStream_t stream, const float* gscale = nullptr);
+
 // ---- FP8 training of the linear layer (gemm_fp8.cu, DESIGN §4.4) ---------------------------------------------
 // Per-tensor power-of-two scaling: amax of a bf16 [rows, cols] matrix (leading dimension ld) -> *amax_bits (the bit
 // pattern of the fp32 amax; zeroed by the caller, atomicMax), then q = fp8(v * s) row-major [rows, cols] and/or

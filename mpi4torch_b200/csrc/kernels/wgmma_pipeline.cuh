@@ -59,9 +59,11 @@ template <int BN> __device__ __forceinline__ void advance(int& stage, uint32_t& 
 }
 
 // Producer: one stage = A rows [m0, m0+128) and B rows [n0, n0+BN) of the k-slice starting at k0.
+// b_row0 is added to B's row coordinate (n for a K-major B, k for an MN-major one): the batched GEMMs read
+// expert e's weights out of one map over the stacked weights with b_row0 = e * (rows of one expert).
 template <bool A_MN, bool B_MN, int BN>
 __device__ __forceinline__ void load_stage(uint8_t* smem, Pipe* p, int& stage, uint32_t& phase, const CUtensorMap* ma,
-                                           const CUtensorMap* mb, int m0, int n0, int k0) {
+                                           const CUtensorMap* mb, int m0, int n0, int k0, int b_row0 = 0) {
   tc::mbar_wait(&p->empty[stage], phase ^ 1);
   uint8_t* sa = smem + stage * Tile<BN>::kStageBytes;
   uint8_t* sb = sa + kABytes;
@@ -74,9 +76,10 @@ __device__ __forceinline__ void load_stage(uint8_t* smem, Pipe* p, int& stage, u
   }
   if (B_MN) {
 #pragma unroll
-    for (int ch = 0; ch < BN / 64; ++ch) tc::tma_load_2d(sb + ch * kBoxBytesMN, mb, &p->full[stage], n0 + ch * 64, k0);
+    for (int ch = 0; ch < BN / 64; ++ch)
+      tc::tma_load_2d(sb + ch * kBoxBytesMN, mb, &p->full[stage], n0 + ch * 64, k0 + b_row0);
   } else {
-    tc::tma_load_2d(sb, mb, &p->full[stage], k0, n0);
+    tc::tma_load_2d(sb, mb, &p->full[stage], k0, n0 + b_row0);
   }
   advance<BN>(stage, phase);
 }

@@ -58,6 +58,7 @@ struct WgradArgs {
   const float* gscale;  // optional device scalar multiplied into every output element (the upstream
                         // gradient of the loss: autograd hands it over as a tensor, never through the host)
   float axpy;           // plain mode with axpy != 0: out <- out + axpy * gscale * G  (single-rank SGD epilogue)
+  int experts;          // BATCHED: E (in the tail padding: the other kernels' parameter layout is unchanged)
 };
 
 struct WgradComm {
@@ -297,7 +298,10 @@ __device__ __forceinline__ void comm_reduce_update(const WgradComm& wc, int firs
 
 // ACC32 (plain mode only): out is an fp32 [N, K] buffer and the epilogue is out <- fmaf(gscale, G, out), the
 // gradient accumulation of micro-batches.  A compile-time mode, so the other instantiations are unchanged.
-template <bool FUSED, bool ACC32 = false>
+// BATCHED (plain mode only): E = g.experts problems G_e = dY_e^T X_e of the same shape, with dY [E Mb, N], X [E Mb, K]
+// and out [E N, K] stacked.  Tile rows of the stacked output run over E * N / 128 blocks: block n_blk belongs to
+// expert n_blk / (N / 128), whose contraction rows start at row expert * Mb of both operands.
+template <bool FUSED, bool ACC32 = false, bool BATCHED = false>
 __global__ void __launch_bounds__(kGemmThreads + (FUSED ? kCommWarps * 32 : 0), 1)
 wgrad_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                         const WgradArgs g, const WgradComm wc) {
@@ -310,7 +314,7 @@ wgrad_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
 
   const int n_tiles = g.N / BM;  // tiles along the rows of G
   const int k_tiles = (g.K + BN - 1) / BN;  // tiles along the columns of G (K % 128 == 0: a last tile may be half)
-  const int num_tiles = n_tiles * k_tiles;
+  const int num_tiles = n_tiles * k_tiles * (BATCHED ? g.experts : 1);
   const UnitSched sched = make_sched(num_tiles, gridDim.x, g.ksplit);
   const int num_units = sched.num_units;
   const int kb_total = g.Mb / BK;
@@ -333,9 +337,10 @@ wgrad_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
         const int kb_per_unit = kb_total / parts;
         const int n_blk = t / k_tiles;
         const int k_blk = t - n_blk * k_tiles;
+        const int expert = BATCHED ? n_blk / n_tiles : 0;
         for (int kb = 0; kb < kb_per_unit; ++kb)
-          load_stage<true, true, BN>(smem, pipe, stage, phase, &tmap_a, &tmap_b, n_blk * BM, k_blk * BN,
-                                 (h * kb_per_unit + kb) * BK);
+          load_stage<true, true, BN>(smem, pipe, stage, phase, &tmap_a, &tmap_b, (n_blk - expert * n_tiles) * BM,
+                                     k_blk * BN, expert * g.Mb + (h * kb_per_unit + kb) * BK);
       }
     }
   } else if (warp < kGemmThreads / 32) {
@@ -444,10 +449,10 @@ CUtensorMap make_tmap_mn(const void* base, int64_t rows, int64_t cols, int64_t l
   return make_tmap_bf16_sw128(base, rows, cols, ld, 64, BK);
 }
 
-template <bool FUSED, bool ACC32 = false> void configure_w() {
+template <bool FUSED, bool ACC32 = false, bool BATCHED = false> void configure_w() {
   static std::once_flag once;
   std::call_once(once, [] {
-    cudaError_t e = cudaFuncSetAttribute(wgrad_bf16_wgmma_kernel<FUSED, ACC32>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(wgrad_bf16_wgmma_kernel<FUSED, ACC32, BATCHED>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          Tile<tile_n<FUSED>()>::kSmemBytes);
     M4T_CHECK(e == cudaSuccess, "cudaFuncSetAttribute(smem) failed: " << cudaGetErrorString(e));
   });
@@ -521,6 +526,38 @@ void launch_wgrad_accumulate(const void* dy, const void* x, float* acc, int64_t 
   cudaError_t e = cudaGetLastError();
   M4T_CHECK(e == cudaSuccess, "wgrad_accumulate launch failed: " << cudaGetErrorString(e));
   note_kernel_launch("wgrad_accumulate");
+}
+
+bool wgrad_bf16_batched_supported(int64_t E, int64_t Mb, int64_t N, int64_t K, const void* dy, const void* x,
+                                  const void* g) {
+  return E > 0 && wgrad_bf16_supported(Mb, N, K, dy, x, g, N, K, K) && E * Mb < (1ll << 31) &&
+         E * N / BM * ((K + tile_n<false>() - 1) / tile_n<false>()) < (1ll << 31);
+}
+
+void launch_wgrad_bf16_batched(const void* dy, const void* x, void* gout, int64_t E, int64_t Mb, int64_t N, int64_t K,
+                               int sm_count, cudaStream_t stream, const float* gscale) {
+  M4T_CHECK(wgrad_bf16_batched_supported(E, Mb, N, K, dy, x, gout),
+            "unsupported shape/alignment for the batched wgrad (N % 128, K % 128, batch % 64, 16-byte-aligned operands)");
+  const CUtensorMap ta = make_tmap_mn(dy, E * Mb, N, N);
+  const CUtensorMap tb = make_tmap_mn(x, E * Mb, K, K);
+  WgradArgs g{};
+  g.out = gout;
+  g.Mb = static_cast<int>(Mb);
+  g.N = static_cast<int>(N);
+  g.K = static_cast<int>(K);
+  g.ldo = static_cast<int>(K);
+  g.ksplit = 1;
+  g.gscale = gscale;
+  g.axpy = 0.0f;
+  g.experts = static_cast<int>(E);
+  constexpr int BN = tile_n<false>();
+  const int64_t tiles = E * (N / BM) * ((K + BN - 1) / BN);
+  const int grid = static_cast<int>(std::max<int64_t>(1, std::min<int64_t>(tiles, sm_count)));
+  configure_w<false, false, true>();
+  wgrad_bf16_wgmma_kernel<false, false, true><<<grid, kGemmThreads, Tile<BN>::kSmemBytes, stream>>>(ta, tb, g, WgradComm{});
+  cudaError_t e = cudaGetLastError();
+  M4T_CHECK(e == cudaSuccess, "wgrad_bf16_batched launch failed: " << cudaGetErrorString(e));
+  note_kernel_launch("wgrad_bf16_batched");
 }
 
 int64_t fused_wgrad_tiles(int64_t N, int64_t K) { return (N / BM) * (K / tile_n<true>()); }
