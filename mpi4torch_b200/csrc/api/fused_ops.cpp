@@ -24,9 +24,25 @@ CudaBackend& backend() {
   return *w.cuda();
 }
 
+cudaStream_t stream_of(const Tensor& t) { return c10::cuda::getCurrentCUDAStream(t.device().index()).stream(); }
+
+int sm_count() { return backend().device_comm().sm_count; }
+
 void check_2d_bf16(const Tensor& t, const char* name) {
   TORCH_CHECK(t.is_cuda() && t.dim() == 2 && t.scalar_type() == at::kBFloat16 && t.stride(1) == 1,
               "mpi4torch_b200: ", name, " must be a 2-d bf16 CUDA tensor with unit inner stride");
+}
+
+// An MSE target [M, N] the GEMM epilogues can read: bf16 with unit inner stride, read as pairs.
+bool mse_target_ok(const Tensor& t, int64_t M, int64_t N) {
+  return t.is_cuda() && t.dim() == 2 && t.scalar_type() == at::kBFloat16 && t.stride(1) == 1 && t.size(0) == M &&
+         t.size(1) == N && epilogue_bf16_pairs_ok(t.data_ptr(), t.stride(0));
+}
+
+// The MSE epilogue against `target`, adding its loss into the fp32 scalar `loss`.
+MseEpilogue mse_epilogue(const Tensor& target, const Tensor& loss, double loss_scale, double grad_scale) {
+  return MseEpilogue{target.data_ptr(), target.stride(0), loss.data_ptr<float>(), static_cast<float>(loss_scale),
+                     static_cast<float>(grad_scale)};
 }
 
 // y = x @ w^T on the wgmma path.
@@ -39,7 +55,7 @@ Tensor gemm_bf16_tn(const Tensor& x, const Tensor& w) {
   if (y.numel() == 0) return y;
   std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
   backend().gemm_bf16_tn(x.data_ptr(), w.data_ptr(), y.data_ptr(), x.size(0), w.size(0), x.size(1), x.stride(0),
-                         w.stride(0), y.stride(0), c10::cuda::getCurrentCUDAStream(x.device().index()).stream());
+                         w.stride(0), y.stride(0), stream_of(x));
   return y;
 }
 
@@ -63,8 +79,7 @@ Tensor gemm_bf16_nn(const Tensor& a, const Tensor& b) {
   if (y.numel() == 0) return y;
   std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
   launch_gemm_bf16_nn(a.data_ptr(), b.data_ptr(), y.data_ptr(), a.size(0), b.size(1), a.size(1), a.stride(0),
-                      b.stride(0), y.stride(0), backend().device_comm().sm_count,
-                      c10::cuda::getCurrentCUDAStream(a.device().index()).stream());
+                      b.stride(0), y.stride(0), sm_count(), stream_of(a));
   return y;
 }
 
@@ -74,11 +89,7 @@ bool gemm_bf16_tn_ok(const Tensor& x, const Tensor& w, const c10::optional<Tenso
   if (!(x.is_cuda() && w.is_cuda() && x.dim() == 2 && w.dim() == 2 && x.scalar_type() == at::kBFloat16 &&
         w.scalar_type() == at::kBFloat16 && x.stride(1) == 1 && w.stride(1) == 1 && x.size(1) == w.size(1)))
     return false;
-  if (target.has_value() &&
-      !(target->is_cuda() && target->dim() == 2 && target->scalar_type() == at::kBFloat16 && target->stride(1) == 1 &&
-        target->size(0) == x.size(0) && target->size(1) == w.size(0) &&
-        epilogue_bf16_pairs_ok(target->data_ptr(), target->stride(0))))
-    return false;
+  if (target.has_value() && !mse_target_ok(*target, x.size(0), w.size(0))) return false;
   if (bias.has_value() && !(bias->is_cuda() && bias->dim() == 1 && bias->scalar_type() == at::kFloat &&
                             bias->is_contiguous() && bias->size(0) == w.size(0) && epilogue_bias_ok(bias->data_ptr<float>())))
     return false;
@@ -104,7 +115,7 @@ std::tuple<Tensor, Tensor> allreduce_linear_fused(const Tensor& x, const Tensor&
   std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
   const void* wavg = backend().fused_allreduce_linear(
       x.data_ptr(), w.data_ptr(), y.data_ptr(), x.size(0), w.size(0), x.size(1), x.stride(0), y.stride(0),
-      static_cast<float>(scale), c10::cuda::getCurrentCUDAStream(x.device().index()).stream());
+      static_cast<float>(scale), stream_of(x));
   Tensor w_avg = torch::from_blob(const_cast<void*>(wavg), {w.size(0), w.size(1)}, w.options());
   return {y, w_avg};
 }
@@ -126,15 +137,10 @@ std::tuple<Tensor, Tensor, Tensor> linear_mse_forward(const Tensor& x, const Ten
   TORCH_CHECK(epilogue_bf16_pairs_ok(target.data_ptr(), target.stride(0)),
               "mpi4torch_b200: the MSE target needs a 4-byte-aligned base and an even row stride");
   c10::cuda::CUDAGuard guard(x.device());
-  cudaStream_t stream = c10::cuda::getCurrentCUDAStream(x.device().index()).stream();
+  cudaStream_t stream = stream_of(x);
   Tensor dy = at::empty({x.size(0), w.size(0)}, x.options());
   Tensor loss = at::zeros({1}, x.options().dtype(at::kFloat));
-  MseEpilogue mse;
-  mse.target = target.data_ptr();
-  mse.ldt = target.stride(0);
-  mse.loss_acc = loss.data_ptr<float>();
-  mse.loss_scale = static_cast<float>(loss_scale);
-  mse.grad_scale = static_cast<float>(grad_scale);
+  const MseEpilogue mse = mse_epilogue(target, loss, loss_scale, grad_scale);
   std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
   CudaBackend& be = backend();
   Tensor w_avg;
@@ -198,8 +204,7 @@ Tensor wgrad_bf16(const Tensor& dy, const Tensor& x, const c10::optional<Tensor>
   Tensor gw = at::empty({dy.size(1), x.size(1)}, x.options());
   std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
   launch_wgrad_bf16(dy.data_ptr(), x.data_ptr(), gw.data_ptr(), dy.size(0), dy.size(1), x.size(1), dy.stride(0),
-                    x.stride(0), gw.stride(0), backend().device_comm().sm_count,
-                    c10::cuda::getCurrentCUDAStream(x.device().index()).stream(), grad_scale_ptr(grad_scale, x));
+                    x.stride(0), gw.stride(0), sm_count(), stream_of(x), grad_scale_ptr(grad_scale, x));
   return gw;
 }
 
@@ -215,8 +220,7 @@ void wgrad_sgd_(Tensor w, const Tensor& dy, const Tensor& x, double scale, const
   c10::cuda::CUDAGuard guard(x.device());
   std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
   launch_wgrad_bf16(dy.data_ptr(), x.data_ptr(), w.data_ptr(), dy.size(0), dy.size(1), x.size(1), dy.stride(0),
-                    x.stride(0), w.stride(0), backend().device_comm().sm_count,
-                    c10::cuda::getCurrentCUDAStream(x.device().index()).stream(), grad_scale_ptr(grad_scale, x),
+                    x.stride(0), w.stride(0), sm_count(), stream_of(x), grad_scale_ptr(grad_scale, x),
                     static_cast<float>(scale));
 }
 
@@ -235,8 +239,8 @@ bool wgrad_accumulate_ok(const Tensor& acc, const Tensor& dy, const Tensor& x) {
   if (!(acc.is_cuda() && acc.device() == x.device() && dy.device() == x.device() && acc.dim() == 2 &&
         acc.scalar_type() == at::kFloat && acc.is_contiguous() && acc.size(0) == dy.size(1) && acc.size(1) == x.size(1)))
     return false;
-  return wgrad_accumulate_supported(dy.size(0), dy.size(1), x.size(1), dy.data_ptr(), x.data_ptr(), acc.data_ptr<float>(),
-                                    dy.stride(0), x.stride(0));
+  return wgrad_bf16_supported(dy.size(0), dy.size(1), x.size(1), dy.data_ptr(), x.data_ptr(), acc.data_ptr<float>(),
+                              dy.stride(0), x.stride(0), x.size(1));
 }
 
 // acc += grad_scale * dy^T @ x, accumulated in fp32 by the wgrad kernel's epilogue with one fmaf per element
@@ -249,8 +253,7 @@ void wgrad_accumulate_(Tensor acc, const Tensor& dy, const Tensor& x, const c10:
   c10::cuda::CUDAGuard guard(x.device());
   std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
   launch_wgrad_accumulate(dy.data_ptr(), x.data_ptr(), acc.data_ptr<float>(), dy.size(0), dy.size(1), x.size(1),
-                          dy.stride(0), x.stride(0), backend().device_comm().sm_count,
-                          c10::cuda::getCurrentCUDAStream(x.device().index()).stream(), grad_scale_ptr(grad_scale, x));
+                          dy.stride(0), x.stride(0), sm_count(), stream_of(x), grad_scale_ptr(grad_scale, x));
 }
 
 bool wgrad_allreduce_sgd_supported(const Tensor& w, const Tensor& dy, const Tensor& x) {
@@ -269,9 +272,7 @@ void wgrad_allreduce_sgd_(Tensor w, const Tensor& dy, const Tensor& x, double sc
   c10::cuda::CUDAGuard guard(x.device());
   std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
   backend().fused_wgrad_update(w.data_ptr(), dy.data_ptr(), x.data_ptr(), dy.size(0), w.size(0), w.size(1), dy.stride(0),
-                               x.stride(0), static_cast<float>(scale),
-                               c10::cuda::getCurrentCUDAStream(x.device().index()).stream(), false,
-                               grad_scale_ptr(grad_scale, x));
+                               x.stride(0), static_cast<float>(scale), stream_of(x), false, grad_scale_ptr(grad_scale, x));
 }
 
 // Same kernel, and additionally the parameter all-reduce of the NEXT forward: returns
@@ -282,9 +283,8 @@ Tensor wgrad_allreduce_sgd_prefetch_(Tensor w, const Tensor& dy, const Tensor& x
   c10::cuda::CUDAGuard guard(x.device());
   std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
   const void* wavg = backend().fused_wgrad_update(w.data_ptr(), dy.data_ptr(), x.data_ptr(), dy.size(0), w.size(0), w.size(1),
-                                                  dy.stride(0), x.stride(0), static_cast<float>(scale),
-                                                  c10::cuda::getCurrentCUDAStream(x.device().index()).stream(), true,
-                                                  grad_scale_ptr(grad_scale, x));
+                                                  dy.stride(0), x.stride(0), static_cast<float>(scale), stream_of(x),
+                                                  true, grad_scale_ptr(grad_scale, x));
   return torch::from_blob(const_cast<void*>(wavg), {w.size(0), w.size(1)}, w.options().requires_grad(false));
 }
 
@@ -298,15 +298,10 @@ std::tuple<Tensor, Tensor> linear_mse_forward_local(const Tensor& x, const Tenso
   TORCH_CHECK(x.size(1) == w_avg.size(1) && target.size(0) == x.size(0) && target.size(1) == w_avg.size(0),
               "mpi4torch_b200: linear_mse_forward_local shape mismatch");
   c10::cuda::CUDAGuard guard(x.device());
-  cudaStream_t stream = c10::cuda::getCurrentCUDAStream(x.device().index()).stream();
+  cudaStream_t stream = stream_of(x);
   Tensor dy = at::empty({x.size(0), w_avg.size(0)}, x.options());
   Tensor loss = at::zeros({1}, x.options().dtype(at::kFloat));
-  MseEpilogue mse;
-  mse.target = target.data_ptr();
-  mse.ldt = target.stride(0);
-  mse.loss_acc = loss.data_ptr<float>();
-  mse.loss_scale = static_cast<float>(loss_scale);
-  mse.grad_scale = static_cast<float>(grad_scale);
+  const MseEpilogue mse = mse_epilogue(target, loss, loss_scale, grad_scale);
   std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
   backend().gemm_bf16_tn(x.data_ptr(), w_avg.data_ptr(), dy.data_ptr(), x.size(0), w_avg.size(0), x.size(1), x.stride(0),
                          w_avg.stride(0), dy.stride(0), stream, &mse);
@@ -336,8 +331,7 @@ std::tuple<Tensor, Tensor> linear_bias_gelu_forward(const Tensor& x, const Tenso
   if (z.numel() == 0) return {h, z};
   std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
   launch_gemm_bias_gelu(x.data_ptr(), w.data_ptr(), b.data_ptr<float>(), z.data_ptr(), h.data_ptr(), x.size(0), w.size(0),
-                        x.size(1), x.stride(0), w.stride(0), z.stride(0), backend().device_comm().sm_count,
-                        c10::cuda::getCurrentCUDAStream(x.device().index()).stream());
+                        x.size(1), x.stride(0), w.stride(0), z.stride(0), sm_count(), stream_of(x));
   return {h, z};
 }
 
@@ -358,16 +352,11 @@ std::tuple<Tensor, Tensor, Tensor> linear_bias_mse_forward_local(const Tensor& x
   Tensor dy = at::empty({x.size(0), w.size(0)}, x.options());
   Tensor loss = at::zeros({1}, x.options().dtype(at::kFloat));
   Tensor part = colsum_workspace(x.size(0), w.size(0), x);
-  MseEpilogue mse;
-  mse.target = target.data_ptr();
-  mse.ldt = target.stride(0);
-  mse.loss_acc = loss.data_ptr<float>();
-  mse.loss_scale = static_cast<float>(loss_scale);
-  mse.grad_scale = static_cast<float>(grad_scale);
+  const MseEpilogue mse = mse_epilogue(target, loss, loss_scale, grad_scale);
   std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
   launch_gemm_bias_mse_colsum(x.data_ptr(), w.data_ptr(), b.data_ptr<float>(), dy.data_ptr(), part.data_ptr<float>(),
                               x.size(0), w.size(0), x.size(1), x.stride(0), w.stride(0), dy.stride(0),
-                              backend().device_comm().sm_count, c10::cuda::getCurrentCUDAStream(x.device().index()).stream(),
+                              sm_count(), stream_of(x),
                               mse);
   return {dy, loss, part};
 }
@@ -398,11 +387,11 @@ std::tuple<Tensor, Tensor, Tensor> linear_bias_xent_forward_local(const Tensor& 
   Tensor ms = at::empty({xent_tiles(C), M, 2}, x.options().dtype(at::kFloat));
   Tensor row_loss = at::empty({M}, x.options().dtype(at::kFloat));
   Tensor done = at::zeros({1}, x.options().dtype(at::kInt));
-  cudaStream_t stream = c10::cuda::getCurrentCUDAStream(x.device().index()).stream();
+  cudaStream_t stream = stream_of(x);
   std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
   float2* ms_ptr = reinterpret_cast<float2*>(ms.data_ptr<float>());
   launch_gemm_bias_xent(x.data_ptr(), w.data_ptr(), b.data_ptr<float>(), dy.data_ptr(), ms_ptr, M, C, x.size(1),
-                        x.stride(0), w.stride(0), dy.stride(0), backend().device_comm().sm_count, stream);
+                        x.stride(0), w.stride(0), dy.stride(0), sm_count(), stream);
   launch_xent_finish(dy.data_ptr(), M, C, dy.stride(0), ms_ptr, labels.data_ptr<int64_t>(), ignore_index,
                      static_cast<float>(loss_scale), static_cast<float>(grad_scale), row_loss.data_ptr<float>(),
                      reinterpret_cast<unsigned int*>(done.data_ptr<int>()), loss.data_ptr<float>(), part.data_ptr<float>(),
@@ -426,8 +415,7 @@ std::tuple<Tensor, Tensor> gemm_nn_gelu_backward(const Tensor& dy, const Tensor&
   std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
   launch_gemm_nn_gelu_bwd_colsum(dy.data_ptr(), w.data_ptr(), z.data_ptr(), dz.data_ptr(), part.data_ptr<float>(), dy.size(0),
                                  w.size(1), dy.size(1), dy.stride(0), w.stride(0), z.stride(0), dz.stride(0),
-                                 backend().device_comm().sm_count,
-                                 c10::cuda::getCurrentCUDAStream(dy.device().index()).stream(), grad_scale_ptr(grad_scale, dy));
+                                 sm_count(), stream_of(dy), grad_scale_ptr(grad_scale, dy));
   return {dz, part};
 }
 
@@ -440,7 +428,7 @@ Tensor column_sum(const Tensor& partials, const c10::optional<Tensor>& grad_scal
   Tensor out = at::empty({partials.size(1)}, partials.options());
   if (out.numel() == 0) return out;
   launch_column_sum(partials.data_ptr<float>(), partials.size(0), partials.size(1), out.data_ptr<float>(),
-                    grad_scale_ptr(grad_scale, partials), c10::cuda::getCurrentCUDAStream(partials.device().index()).stream());
+                    grad_scale_ptr(grad_scale, partials), stream_of(partials));
   return out;
 }
 
@@ -483,10 +471,6 @@ bool batched_wgrad_bf16_ok(const Tensor& dy, const Tensor& x) {
   return World::instance().cuda_ready() && wgrad_bf16_batched_supported(dy.size(0), dy.size(1), dy.size(2), x.size(2),
                                                                          dy.data_ptr(), x.data_ptr(), x.data_ptr());
 }
-
-cudaStream_t stream_of(const Tensor& t) { return c10::cuda::getCurrentCUDAStream(t.device().index()).stream(); }
-
-int sm_count() { return backend().device_comm().sm_count; }
 
 // (h, z) per expert: z_e = x_e @ w_e^T + b_e, h_e = gelu_tanh(z_e), as linear_bias_gelu_forward, in one launch.
 std::tuple<Tensor, Tensor> batched_linear_bias_gelu_forward(const Tensor& x, const Tensor& w, const Tensor& b) {
@@ -597,7 +581,7 @@ std::tuple<Tensor, Tensor, Tensor> quantize_fp8(const Tensor& x, c10::string_vie
   TORCH_CHECK(!given || (scalar_ok(*amax, x) && amax->is_contiguous()),
               "mpi4torch_b200: amax must be a one-element fp32 tensor on x's device");
   c10::cuda::CUDAGuard guard(x.device());
-  cudaStream_t stream = c10::cuda::getCurrentCUDAStream(x.device().index()).stream();
+  cudaStream_t stream = stream_of(x);
   const auto dt = e5m2 ? at::kFloat8_e5m2 : at::kFloat8_e4m3fn;
   const int64_t R = x.size(0), C = x.size(1);
   Tensor q = rowwise ? at::empty({R, C}, x.options().dtype(dt)) : Tensor();
@@ -606,7 +590,7 @@ std::tuple<Tensor, Tensor, Tensor> quantize_fp8(const Tensor& x, c10::string_vie
   std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
   Tensor am = given ? *amax : at::zeros({1}, x.options().dtype(at::kFloat));
   auto* bits = reinterpret_cast<unsigned int*>(am.data_ptr<float>());
-  if (!given) launch_quantize_fp8_amax(x.data_ptr(), R, C, x.stride(0), bits, backend().device_comm().sm_count, stream);
+  if (!given) launch_quantize_fp8_amax(x.data_ptr(), R, C, x.stride(0), bits, sm_count(), stream);
   launch_quantize_fp8_cast(x.data_ptr(), R, C, x.stride(0), e5m2, bits, rowwise ? q.data_ptr() : nullptr,
                            transposed ? qt.data_ptr() : nullptr, si.data_ptr<float>(), stream);
   return {q, qt, si};
@@ -622,9 +606,7 @@ bool gemm_fp8_tn_ok(const Tensor& a, const Tensor& b, const Tensor& a_si, const 
         scalar_ok(a_si, a) && scalar_ok(b_si, a)))
     return false;
   if (target.has_value() && target->defined() &&
-      !(target->is_cuda() && target->device() == a.device() && target->dim() == 2 &&
-        target->scalar_type() == at::kBFloat16 && target->stride(1) == 1 && target->size(0) == a.size(0) &&
-        target->size(1) == b.size(0) && epilogue_bf16_pairs_ok(target->data_ptr(), target->stride(0))))
+      !(target->device() == a.device() && mse_target_ok(*target, a.size(0), b.size(0))))
     return false;
   const void* c = a.data_ptr();
   int64_t ldc = b.size(0);
@@ -652,8 +634,7 @@ Tensor gemm_fp8_tn(const Tensor& a, const Tensor& b, const Tensor& a_si, const T
   std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
   launch_gemm_fp8_tn(a.data_ptr(), a.scalar_type() == at::kFloat8_e5m2, b.data_ptr(), c.data_ptr(), a.size(0), b.size(0),
                      a.size(1), a.stride(0), b.stride(0), c.stride(0), a_si.data_ptr<float>(), b_si.data_ptr<float>(),
-                     grad_scale_ptr(grad_scale, a), backend().device_comm().sm_count,
-                     c10::cuda::getCurrentCUDAStream(a.device().index()).stream());
+                     grad_scale_ptr(grad_scale, a), sm_count(), stream_of(a));
   return c;
 }
 
@@ -671,17 +652,11 @@ std::tuple<Tensor, Tensor, Tensor> linear_mse_forward_fp8_local(const Tensor& xq
   Tensor dy = at::empty({xq.size(0), wq.size(0)}, xq.options().dtype(at::kBFloat16));
   Tensor loss = at::zeros({1}, xq.options().dtype(at::kFloat));
   Tensor amax = at::zeros({1}, xq.options().dtype(at::kFloat));
-  MseEpilogue mse;
-  mse.target = target.data_ptr();
-  mse.ldt = target.stride(0);
-  mse.loss_acc = loss.data_ptr<float>();
-  mse.loss_scale = static_cast<float>(loss_scale);
-  mse.grad_scale = static_cast<float>(grad_scale);
+  const MseEpilogue mse = mse_epilogue(target, loss, loss_scale, grad_scale);
   std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
   launch_gemm_fp8_mse(xq.data_ptr(), wq.data_ptr(), dy.data_ptr(), xq.size(0), wq.size(0), xq.size(1), xq.stride(0),
                       wq.stride(0), dy.stride(0), x_si.data_ptr<float>(), w_si.data_ptr<float>(), mse,
-                      reinterpret_cast<unsigned int*>(amax.data_ptr<float>()), backend().device_comm().sm_count,
-                      c10::cuda::getCurrentCUDAStream(xq.device().index()).stream());
+                      reinterpret_cast<unsigned int*>(amax.data_ptr<float>()), sm_count(), stream_of(xq));
   return {dy, loss, amax};
 }
 
@@ -696,8 +671,7 @@ void gemm_fp8_tn_sgd_(Tensor w, const Tensor& a, const Tensor& b, const Tensor& 
   std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
   launch_gemm_fp8_sgd(a.data_ptr(), a.scalar_type() == at::kFloat8_e5m2, b.data_ptr(), w.data_ptr(), a.size(0), b.size(0),
                       a.size(1), a.stride(0), b.stride(0), w.stride(0), a_si.data_ptr<float>(), b_si.data_ptr<float>(),
-                      static_cast<float>(scale), grad_scale_ptr(grad_scale, a), backend().device_comm().sm_count,
-                      c10::cuda::getCurrentCUDAStream(a.device().index()).stream());
+                      static_cast<float>(scale), grad_scale_ptr(grad_scale, a), sm_count(), stream_of(a));
 }
 
 }  // namespace

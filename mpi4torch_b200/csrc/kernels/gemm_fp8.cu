@@ -14,9 +14,6 @@
 #include <cuda.h>
 #include <cuda_fp8.h>
 
-#include <algorithm>
-#include <mutex>
-
 #include "kernels.h"
 #include "tma_host.h"
 #include "wgmma_pipeline.cuh"
@@ -285,20 +282,10 @@ __global__ void __launch_bounds__(kQThreads) quantize_fp8_cast_kernel(const uint
 template <int EPI, bool A_E5M2>
 void launch_fp8(const Fp8Args& g, const void* A, const void* B, int64_t lda, int64_t ldb, int sm_count,
                 cudaStream_t stream, const char* what) {
-  static std::once_flag once;
-  std::call_once(once, [] {
-    cudaError_t e = cudaFuncSetAttribute(gemm_fp8_kernel<EPI, A_E5M2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Tile<BN8>::kSmemBytes);
-    M4T_CHECK(e == cudaSuccess, "cudaFuncSetAttribute(smem) failed: " << cudaGetErrorString(e));
-  });
-  const CUtensorMap ta = make_tmap_u8_sw128(A, g.M, g.K, lda, BM);
-  const CUtensorMap tb = make_tmap_u8_sw128(B, g.N, g.K, ldb, BN8);
   const int64_t tiles = ((g.M + BM - 1) / BM) * ((g.N + BN8 - 1) / BN8);
-  const int grid = static_cast<int>(std::max<int64_t>(1, std::min<int64_t>(tiles, sm_count)));
-  gemm_fp8_kernel<EPI, A_E5M2><<<grid, kGemmThreads, Tile<BN8>::kSmemBytes, stream>>>(ta, tb, g);
-  cudaError_t err = cudaGetLastError();
-  M4T_CHECK(err == cudaSuccess, what << " launch failed: " << cudaGetErrorString(err));
-  note_kernel_launch(what);
+  launch_kernel<gemm_fp8_kernel<EPI, A_E5M2>>(persistent_grid(tiles, sm_count), kGemmThreads, Tile<BN8>::kSmemBytes,
+                                              stream, what, make_tmap_u8_sw128(A, g.M, g.K, lda, BM),
+                                              make_tmap_u8_sw128(B, g.N, g.K, ldb, BN8), g);
 }
 
 template <int EPI>
@@ -320,15 +307,13 @@ Fp8Args fp8_args(void* C, int64_t M, int64_t N, int64_t K, int64_t ldc, const fl
   return g;
 }
 
-bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
-
 }  // namespace
 
 bool gemm_fp8_tn_supported(int64_t M, int64_t N, int64_t K, const void* A, const void* B, const void* C, int64_t lda,
                            int64_t ldb, int64_t ldc) {
   return M > 0 && N > 0 && K > 0 && K % 16 == 0 && N % 8 == 0 && lda % 16 == 0 && ldb % 16 == 0 && ldc % 8 == 0 &&
-         lda >= K && ldb >= K && ldc >= N && al16(A) && al16(B) && al16(C) && M < (1ll << 31) && N < (1ll << 31) &&
-         K < (1ll << 31) && ldc < (1ll << 31);
+         lda >= K && ldb >= K && ldc >= N && aligned16(A) && aligned16(B) && aligned16(C) && M < (1ll << 31) &&
+         N < (1ll << 31) && K < (1ll << 31) && ldc < (1ll << 31);
 }
 
 void launch_gemm_fp8_tn(const void* A, bool a_e5m2, const void* B, void* C, int64_t M, int64_t N, int64_t K, int64_t lda,
@@ -365,7 +350,7 @@ void launch_gemm_fp8_sgd(const void* A, bool a_e5m2, const void* B, void* W, int
   dispatch_fp8<kSgd>(g, a_e5m2, A, B, lda, ldb, sm_count, stream, "gemm_fp8_sgd");
 }
 
-bool quantize_fp8_vec_ok(const void* x, int64_t cols, int64_t ld) { return al16(x) && cols % 8 == 0 && ld % 8 == 0; }
+bool quantize_fp8_vec_ok(const void* x, int64_t cols, int64_t ld) { return aligned16(x) && cols % 8 == 0 && ld % 8 == 0; }
 
 void launch_quantize_fp8_amax(const void* x, int64_t rows, int64_t cols, int64_t ld, unsigned int* amax_bits,
                               int sm_count, cudaStream_t stream) {
@@ -374,33 +359,28 @@ void launch_quantize_fp8_amax(const void* x, int64_t rows, int64_t cols, int64_t
   const int64_t work = vec ? rows * (cols / 8) : rows * cols;
   const int blocks = static_cast<int>(std::max<int64_t>(1, std::min<int64_t>((work + kQThreads - 1) / kQThreads,
                                                                              static_cast<int64_t>(sm_count) * 8)));
-  quantize_fp8_amax_kernel<<<blocks, kQThreads, 0, stream>>>(static_cast<const uint16_t*>(x), rows, cols, ld, vec,
-                                                             amax_bits);
-  cudaError_t err = cudaGetLastError();
-  M4T_CHECK(err == cudaSuccess, "quantize_fp8_amax launch failed: " << cudaGetErrorString(err));
-  note_kernel_launch("quantize_fp8_amax");
+  launch_kernel<quantize_fp8_amax_kernel>(blocks, kQThreads, 0, stream, "quantize_fp8_amax",
+                                          static_cast<const uint16_t*>(x), rows, cols, ld, vec, amax_bits);
 }
 
 void launch_quantize_fp8_cast(const void* x, int64_t rows, int64_t cols, int64_t ld, bool e5m2,
                               const unsigned int* amax_bits, void* q, void* qt, float* scale_inv, cudaStream_t stream) {
   M4T_CHECK(rows > 0 && cols > 0 && ld >= cols, "quantize_fp8: empty matrix or bad leading dimension");
   M4T_CHECK(q == nullptr || cols % 8 != 0 || (reinterpret_cast<uintptr_t>(q) & 7u) == 0, "quantize_fp8: q misaligned");
-  M4T_CHECK(qt == nullptr || al16(qt), "quantize_fp8: qt misaligned");
+  M4T_CHECK(qt == nullptr || aligned16(qt), "quantize_fp8: qt misaligned");
   const int64_t bx = (cols + kQTile - 1) / kQTile, by = (rows + kQTile - 1) / kQTile;
   M4T_CHECK(bx < (1ll << 31) && by < 65536, "quantize_fp8: matrix too large");
   const dim3 grid(static_cast<unsigned>(bx), static_cast<unsigned>(by));
   const bool vec = quantize_fp8_vec_ok(x, cols, ld);
+  const auto* xb = static_cast<const uint16_t*>(x);
   auto* qb = static_cast<uint8_t*>(q);
   auto* qtb = static_cast<uint8_t*>(qt);
   if (e5m2)
-    quantize_fp8_cast_kernel<true><<<grid, kQThreads, 0, stream>>>(static_cast<const uint16_t*>(x), rows, cols, ld, vec,
-                                                                   amax_bits, qb, qtb, scale_inv);
+    launch_kernel<quantize_fp8_cast_kernel<true>>(grid, kQThreads, 0, stream, "quantize_fp8_cast", xb, rows, cols, ld,
+                                                  vec, amax_bits, qb, qtb, scale_inv);
   else
-    quantize_fp8_cast_kernel<false><<<grid, kQThreads, 0, stream>>>(static_cast<const uint16_t*>(x), rows, cols, ld, vec,
-                                                                    amax_bits, qb, qtb, scale_inv);
-  cudaError_t err = cudaGetLastError();
-  M4T_CHECK(err == cudaSuccess, "quantize_fp8_cast launch failed: " << cudaGetErrorString(err));
-  note_kernel_launch("quantize_fp8_cast");
+    launch_kernel<quantize_fp8_cast_kernel<false>>(grid, kQThreads, 0, stream, "quantize_fp8_cast", xb, rows, cols, ld,
+                                                   vec, amax_bits, qb, qtb, scale_inv);
 }
 
 }  // namespace m4t

@@ -12,9 +12,6 @@
 // all-reduce of panel p+1.. overlaps the MMAs on panel p.
 #include <cuda.h>
 
-#include <algorithm>
-#include <mutex>
-
 #include "kernels.h"
 #include "fused_comm.cuh"
 #include "tma_host.h"
@@ -27,13 +24,23 @@ namespace {
 using namespace wg;
 
 constexpr int kPanel = 256;  // weight rows per all-reduce panel of the fused kernel (one counter each)
-constexpr int kCommWarps = 4;
+
+// Epilogues of gemm_bf16_wgmma_kernel, its EPI template argument (an int, so the kernels' symbol names stay plain):
+//   kStore          C = acc
+//   kMse            C = grad_scale * (acc - T), loss_scale * sum((acc - T)^2) added to *loss_acc
+//   kBiasGelu ...   the MLP epilogues, see mlp_epilogue and xent_epilogue
+enum : int { kStore = 0, kMse = 1, kBiasGelu = 2, kBiasMseColsum = 3, kGeluBwdColsum = 4, kBiasXent = 5, kBias = 6 };
+constexpr bool epi_adds_loss(int epi) { return epi == kMse || epi == kBiasMseColsum; }
+constexpr bool epi_reads_t(int epi) { return epi == kMse || epi == kBiasMseColsum || epi == kGeluBwdColsum; }
+// The MLP epilogues hold bias, target / z values and column sums next to the accumulators: the producer warpgroup
+// hands registers to the consumers (40 + 2 x 232 per thread fits the register file).
+constexpr bool epi_reallocs(int epi) { return epi >= kBiasGelu; }
 
 struct GemmArgs {
   void* C;
   int M, N, K;
   int ldc;
-  // fused MSE epilogue (EPI == 1): C receives dL/dy = grad_scale * (y - T),
+  // fused MSE epilogue (kMse): C receives dL/dy = grad_scale * (y - T),
   // loss_acc accumulates loss_scale * sum((y - T)^2); y itself is never stored
   const void* T;
   int ldt;
@@ -47,23 +54,20 @@ struct GemmArgs {
   int expert_rows;
 };
 
-// the fused kernel's communication warps need registers: half-width tiles there
-template <bool FUSED> constexpr int tile_n() { return FUSED ? 128 : 256; }
-
-// Epilogues of the two-layer MLP (EPI 2..5; unused by EPI 0/1):
-//   EPI 2  TN  z = acc + bias -> C,  h = gelu_tanh(z) -> h_out
-//   EPI 3  TN  d = acc + bias - T:  C = grad_scale * d, loss as EPI 1, column-sum partials of C
-//   EPI 4  NN  C = gscale * acc * gelu_tanh'(z), z read from T (bf16), column-sum partials of C
-//   EPI 5  TN  C = logits = acc + bias, per-tile softmax partials (xent_epilogue; xent_finish completes them)
-//   EPI 6  TN  C = acc + bias (EPI 2 without h)
+// Epilogues of the two-layer MLP (unused by kStore / kMse):
+//   kBiasGelu       TN  z = acc + bias -> C,  h = gelu_tanh(z) -> h_out
+//   kBiasMseColsum  TN  d = acc + bias - T:  C = grad_scale * d, loss as kMse, column-sum partials of C
+//   kGeluBwdColsum  NN  C = gscale * acc * gelu_tanh'(z), z read from T (bf16), column-sum partials of C
+//   kBiasXent       TN  C = logits = acc + bias, per-tile softmax partials (xent_epilogue; xent_finish completes them)
+//   kBias           TN  C = acc + bias (kBiasGelu without h)
 // Column sums are deterministic: a warp adds its 16 rows in registers (h pair, then lane bits 2-4) and
 // lanes 0-3 store one fp32 row of colsum[ceil(M/16), N]; column_sum_kernel adds those rows in a fixed order.
 struct MlpEpiArgs {
   const float* bias;    // [N] fp32
-  void* h_out;          // EPI 2: bf16, same layout as C
-  float* colsum;        // EPI 3, 4: [ceil(M/16), N] fp32, row-major
-  const float* gscale;  // EPI 4: optional device scalar
-  float2* xent_ms;      // EPI 5: [ceil(N/256), M] (max, sum of exp) per row and column tile
+  void* h_out;          // kBiasGelu: bf16, same layout as C
+  float* colsum;        // kBiasMseColsum, kGeluBwdColsum: [ceil(M/16), N] fp32, row-major
+  const float* gscale;  // kGeluBwdColsum: optional device scalar
+  float2* xent_ms;      // kBiasXent: [ceil(N/256), M] (max, sum of exp) per row and column tile
 };
 
 constexpr float kGeluBeta = 0.7978845608028654f;  // sqrt(2/pi)
@@ -81,17 +85,60 @@ __device__ __forceinline__ float gelu_tanh_grad(float v) {
   return 0.5f * (1.f + t) + 0.5f * v * (1.f - t * t) * kGeluBeta * fmaf(3.f * kGeluKappa, v2, 1.f);
 }
 
-// Epilogue of one consumer warpgroup's 64 x BN accumulators for EPI 2..4.  Column pairs are handled in
-// groups of kGroup, small enough that the bias / target / z values and the column sums fit next to acc.
+// Epilogue of one consumer warpgroup's 64 x BN accumulators for kStore and kMse; returns this thread's part of the
+// kMse loss.  N is a multiple of 8, so a column pair is either wholly inside or wholly outside.
+template <int EPI, int BN>
+__device__ __forceinline__ float store_epilogue(const float (&acc)[BN / 2], const GemmArgs& g, int m_blk, int n_blk,
+                                                int wgi) {
+  float loss_part = 0.f;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = m_blk * BM + wgi * 64 + frag_row(h);
+    if (row >= g.M) continue;
+    uint16_t* crow = static_cast<uint16_t*>(g.C) + static_cast<int64_t>(row) * g.ldc;
+    const uint16_t* trow = epi_reads_t(EPI) ? static_cast<const uint16_t*>(g.T) + static_cast<int64_t>(row) * g.ldt : nullptr;
+#pragma unroll
+    for (int j0 = 0; j0 < BN / 8; j0 += 8) {
+      uint32_t tv[8];  // the targets of eight column pairs are requested before the first is used
+      if (epi_reads_t(EPI)) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int col = n_blk * BN + frag_col(j0 + j);
+          tv[j] = col < g.N ? __ldcs(reinterpret_cast<const unsigned int*>(trow + col)) : 0u;
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int col = n_blk * BN + frag_col(j0 + j);
+        if (col >= g.N) continue;
+        float v0 = acc[4 * (j0 + j) + 2 * h], v1 = acc[4 * (j0 + j) + 2 * h + 1];
+        if (EPI == kMse) {
+          const float d0 = v0 - bf16_bits_to_float(static_cast<uint16_t>(tv[j] & 0xffffu));
+          const float d1 = v1 - bf16_bits_to_float(static_cast<uint16_t>(tv[j] >> 16));
+          loss_part = fmaf(d0, d0, loss_part);
+          loss_part = fmaf(d1, d1, loss_part);
+          v0 = d0 * g.grad_scale;
+          v1 = d1 * g.grad_scale;
+        }
+        *reinterpret_cast<uint32_t*>(crow + col) = pack_bf16x2(v0, v1);
+      }
+    }
+  }
+  return loss_part;
+}
+
+// Epilogue of one consumer warpgroup's 64 x BN accumulators for kBiasGelu, kBiasMseColsum, kGeluBwdColsum and kBias.
+// Column pairs are handled in groups of kGroup, small enough that the bias / target / z values and the column sums
+// fit next to acc.
 template <int EPI, int BN>
 __device__ __forceinline__ void mlp_epilogue(const float (&acc)[BN / 2], const GemmArgs& g, const MlpEpiArgs& e,
                                              int m_blk, int n_blk, int wgi, float& loss_part) {
   constexpr int kGroup = 4;
-  constexpr bool kBias = EPI != 4, kReadT = EPI == 3 || EPI == 4, kColsum = EPI == 3 || EPI == 4;
+  constexpr bool kAddBias = EPI != kGeluBwdColsum, kColsum = EPI == kBiasMseColsum || EPI == kGeluBwdColsum;
   const int lane = threadIdx.x & 31;
   const int row0 = m_blk * BM + wgi * 64 + frag_row(0);
   const bool row_ok[2] = {row0 < g.M, row0 + 8 < g.M};
-  const float gs = (EPI == 4 && e.gscale != nullptr) ? *e.gscale : 1.f;
+  const float gs = (EPI == kGeluBwdColsum && e.gscale != nullptr) ? *e.gscale : 1.f;
   const int prow = (m_blk * BM + wgi * 64) / 16 + ((threadIdx.x >> 5) & 3);  // this warp's colsum row
 #pragma unroll
   for (int j0 = 0; j0 < BN / 8; j0 += kGroup) {
@@ -103,8 +150,8 @@ __device__ __forceinline__ void mlp_epilogue(const float (&acc)[BN / 2], const G
     for (int j = 0; j < kGroup; ++j) {
       const int col = n_blk * BN + frag_col(j0 + j);
       const bool col_ok = col < g.N;
-      if (kBias) bv[j] = col_ok ? *reinterpret_cast<const float2*>(e.bias + col) : make_float2(0.f, 0.f);
-      if (kReadT) {
+      if (kAddBias) bv[j] = col_ok ? *reinterpret_cast<const float2*>(e.bias + col) : make_float2(0.f, 0.f);
+      if (epi_reads_t(EPI)) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const uint16_t* trow = static_cast<const uint16_t*>(g.T) + static_cast<int64_t>(row0 + 8 * h) * g.ldt;
@@ -121,7 +168,7 @@ __device__ __forceinline__ void mlp_epilogue(const float (&acc)[BN / 2], const G
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         float v0 = acc[4 * (j0 + j) + 2 * h], v1 = acc[4 * (j0 + j) + 2 * h + 1];
-        if (kBias) {
+        if (kAddBias) {
           v0 += bv[j].x;
           v1 += bv[j].y;
         }
@@ -129,15 +176,15 @@ __device__ __forceinline__ void mlp_epilogue(const float (&acc)[BN / 2], const G
         const int64_t off = static_cast<int64_t>(row0 + 8 * h) * g.ldc + col;
         const float t0 = bf16_bits_to_float(static_cast<uint16_t>(tv[h][j] & 0xffffu));
         const float t1 = bf16_bits_to_float(static_cast<uint16_t>(tv[h][j] >> 16));
-        if (EPI == 2) {
+        if (EPI == kBiasGelu) {
           *reinterpret_cast<uint32_t*>(static_cast<uint16_t*>(e.h_out) + off) = pack_bf16x2(gelu_tanh(v0), gelu_tanh(v1));
-        } else if (EPI == 3) {
+        } else if (EPI == kBiasMseColsum) {
           const float d0 = v0 - t0, d1 = v1 - t1;
           loss_part = fmaf(d0, d0, loss_part);
           loss_part = fmaf(d1, d1, loss_part);
           v0 = d0 * g.grad_scale;
           v1 = d1 * g.grad_scale;
-        } else if (EPI == 4) {
+        } else if (EPI == kGeluBwdColsum) {
           v0 = gs * v0 * gelu_tanh_grad(t0);
           v1 = gs * v1 * gelu_tanh_grad(t1);
         }
@@ -166,7 +213,7 @@ __device__ __forceinline__ void mlp_epilogue(const float (&acc)[BN / 2], const G
 // the same function, or the softmax of a row would not add up to one.
 __device__ __forceinline__ float xent_exp(float v) { return expf(v); }
 
-// EPI 5  TN  logit = bf16(acc + bias) -> C, and for each row the pair (m, s) of this 256-column tile: m the max of
+// kBiasXent  TN  logit = bf16(acc + bias) -> C, and for each row the pair (m, s) of this 256-column tile: m the max of
 // the row's stored (bf16-rounded) logits over the valid columns, s = sum exp(logit - m).  A thread reduces its 64
 // values of a row, the quad (lanes 4r .. 4r+3 hold one row) combines them, and its first lane stores the pair.
 // A -inf logit adds nothing to s without evaluating exp: a tile of -inf gives (-inf, 0), never exp(-inf - -inf).
@@ -246,12 +293,9 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
   }
   __syncthreads();
 
-  // The MLP epilogues hold bias, target / z values and column sums next to the accumulators: the
-  // producer warpgroup hands registers to the consumers (40 + 2 x 232 per thread fits the register file).
-  constexpr bool kRealloc = EPI >= 2;
   if (warp < 4) {
     // =========================== TMA producer ===========================
-    if constexpr (kRealloc) tc::setmaxnreg_dec<40>();
+    if constexpr (epi_reallocs(EPI)) tc::setmaxnreg_dec<40>();
     if (warp == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -271,7 +315,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     }
   } else if (warp < kGemmThreads / 32) {
     // ====================== consumers: wgmma + epilogue ======================
-    if constexpr (kRealloc) tc::setmaxnreg_inc<232>();
+    if constexpr (epi_reallocs(EPI)) tc::setmaxnreg_inc<232>();
     const int wgi = warp / 4 - 1;
     int stage = 0;
     uint32_t phase = 0;
@@ -281,51 +325,18 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
       const int m_blk = t - n_blk * m_tiles;
       mma_tile<false, B_MN, BN>(acc, smem, pipe, stage, phase, k_blocks, wgi);
       float loss_part = 0.f;
-      if constexpr (EPI == 5) {
+      if constexpr (EPI == kStore || EPI == kMse) {
+        loss_part = store_epilogue<EPI, BN>(acc, g, m_blk, n_blk, wgi);
+      } else if constexpr (EPI == kBiasXent) {
         xent_epilogue<BN>(acc, g, e, m_blk, n_blk, wgi);
-      } else if constexpr (EPI >= 2 && BATCHED) {
+      } else if constexpr (BATCHED) {
         MlpEpiArgs ex = e;
         if (e.bias != nullptr) ex.bias = e.bias + static_cast<int64_t>(m_blk * BM / g.expert_rows) * g.N;
         mlp_epilogue<EPI, BN>(acc, g, ex, m_blk, n_blk, wgi, loss_part);
-      } else if constexpr (EPI >= 2) {
-        mlp_epilogue<EPI, BN>(acc, g, e, m_blk, n_blk, wgi, loss_part);
       } else {
-  #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int row = m_blk * BM + wgi * 64 + frag_row(h);
-          if (row >= g.M) continue;
-          uint16_t* crow = static_cast<uint16_t*>(g.C) + static_cast<int64_t>(row) * g.ldc;
-          const uint16_t* trow = EPI == 1 ? static_cast<const uint16_t*>(g.T) + static_cast<int64_t>(row) * g.ldt : nullptr;
-          // N is a multiple of 8, so a column pair is either wholly inside or wholly outside
-  #pragma unroll
-          for (int j0 = 0; j0 < BN / 8; j0 += 8) {
-            uint32_t tv[8];  // the targets of eight column pairs are requested before the first is used
-            if (EPI == 1) {
-  #pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const int col = n_blk * BN + frag_col(j0 + j);
-                tv[j] = col < g.N ? __ldcs(reinterpret_cast<const unsigned int*>(trow + col)) : 0u;
-              }
-            }
-  #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const int col = n_blk * BN + frag_col(j0 + j);
-              if (col >= g.N) continue;
-              float v0 = acc[4 * (j0 + j) + 2 * h], v1 = acc[4 * (j0 + j) + 2 * h + 1];
-              if (EPI == 1) {
-                const float d0 = v0 - bf16_bits_to_float(static_cast<uint16_t>(tv[j] & 0xffffu));
-                const float d1 = v1 - bf16_bits_to_float(static_cast<uint16_t>(tv[j] >> 16));
-                loss_part = fmaf(d0, d0, loss_part);
-                loss_part = fmaf(d1, d1, loss_part);
-                v0 = d0 * g.grad_scale;
-                v1 = d1 * g.grad_scale;
-              }
-              *reinterpret_cast<uint32_t*>(crow + col) = pack_bf16x2(v0, v1);
-            }
-          }
-        }
+        mlp_epilogue<EPI, BN>(acc, g, e, m_blk, n_blk, wgi, loss_part);
       }
-      if (EPI == 1 || EPI == 3) {
+      if (epi_adds_loss(EPI)) {
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) loss_part += __shfl_xor_sync(0xffffffffu, loss_part, o);
         if (lane == 0) atomicAdd(g.loss_acc, loss_part * g.loss_scale);
@@ -346,26 +357,16 @@ CUtensorMap make_tmap(const void* base, int64_t rows, int64_t cols, int64_t ld, 
   return make_tmap_bf16_sw128(base, rows, cols, ld, BK, box_rows);
 }
 
-template <bool FUSED> constexpr int smem_bytes() { return Tile<tile_n<FUSED>()>::kSmemBytes; }
-
-template <bool FUSED, int EPI, bool B_MN, bool BATCHED> void configure_once() {
-  static std::once_flag once;
-  std::call_once(once, [] {
-    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<FUSED, EPI, B_MN, BATCHED>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes<FUSED>());
-    M4T_CHECK(e == cudaSuccess, "cudaFuncSetAttribute(smem) failed: " << cudaGetErrorString(e));
-  });
-}
-
+// ctas: the SM count, of which the persistent grid uses no more than g has tiles; the fused kernel's grid
+// (fused_gemm_grid), which it uses whole.
 template <bool FUSED, int EPI, bool B_MN, bool BATCHED = false>
-void launch(int grid, const CUtensorMap& ta, const CUtensorMap& tb, const GemmArgs& g, const CommArgs& cm,
-            cudaStream_t stream, const char* what, const MlpEpiArgs& e = MlpEpiArgs{}) {
-  configure_once<FUSED, EPI, B_MN, BATCHED>();
-  gemm_bf16_wgmma_kernel<FUSED, EPI, B_MN, BATCHED>
-      <<<grid, kGemmThreads + (FUSED ? kCommWarps * 32 : 0), smem_bytes<FUSED>(), stream>>>(ta, tb, g, cm, e);
-  cudaError_t err = cudaGetLastError();
-  M4T_CHECK(err == cudaSuccess, what << " launch failed: " << cudaGetErrorString(err));
-  note_kernel_launch(what);
+void launch(int ctas, const CUtensorMap& ta, const CUtensorMap& tb, const GemmArgs& g, cudaStream_t stream,
+            const char* what, const MlpEpiArgs& e = MlpEpiArgs{}, const CommArgs& cm = CommArgs{}) {
+  constexpr int BN = tile_n<FUSED>();
+  const int64_t M = g.M, N = g.N;
+  const int grid = FUSED ? ctas : persistent_grid(((M + BM - 1) / BM) * ((N + BN - 1) / BN), ctas);
+  launch_kernel<gemm_bf16_wgmma_kernel<FUSED, EPI, B_MN, BATCHED>>(grid, kGemmThreads + (FUSED ? kCommWarps * 32 : 0),
+                                                                     Tile<BN>::kSmemBytes, stream, what, ta, tb, g, cm, e);
 }
 
 void set_mse(GemmArgs& g, const MseEpilogue* mse) {
@@ -531,20 +532,19 @@ GemmArgs plain_args(void* C, int64_t M, int64_t N, int64_t K, int64_t ldc) {
   return g;
 }
 
-int plain_grid(int64_t M, int64_t N, int sm_count) {
-  constexpr int BN = tile_n<false>();
-  const int tiles = static_cast<int>(((M + BM - 1) / BM) * ((N + BN - 1) / BN));
-  return std::max(1, std::min(tiles, sm_count));
+GemmArgs batched_args(void* C, int64_t E, int64_t M, int64_t N, int64_t K) {
+  GemmArgs g = plain_args(C, E * M, N, K, N);
+  g.expert_rows = static_cast<int>(M);
+  return g;
 }
 
 }  // namespace
 
 bool gemm_bf16_tn_supported(int64_t M, int64_t N, int64_t K, const void* A, const void* B, const void* C, int64_t lda,
                             int64_t ldb, int64_t ldc) {
-  auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
   return M > 0 && N > 0 && K > 0 && (K % 8) == 0 && (N % 8) == 0 && (lda % 8) == 0 && (ldb % 8) == 0 && (ldc % 8) == 0 &&
-         lda >= K && ldb >= K && ldc >= N && al16(A) && al16(B) && al16(C) && M < (1ll << 31) && N < (1ll << 31) &&
-         K < (1ll << 31);
+         lda >= K && ldb >= K && ldc >= N && aligned16(A) && aligned16(B) && aligned16(C) && M < (1ll << 31) &&
+         N < (1ll << 31) && K < (1ll << 31);
 }
 
 bool epilogue_bf16_pairs_ok(const void* p, int64_t ld) {
@@ -558,48 +558,31 @@ void launch_gemm_bf16_tn(const void* A, const void* B, void* C, int64_t M, int64
   M4T_CHECK(gemm_bf16_tn_supported(M, N, K, A, B, C, lda, ldb, ldc), "unsupported GEMM shape/alignment for the wgmma path");
   M4T_CHECK(mse == nullptr || epilogue_bf16_pairs_ok(mse->target, mse->ldt),
             "the MSE target needs a 4-byte-aligned base and an even row stride");
-  constexpr int BN = tile_n<false>();
   const CUtensorMap ta = make_tmap(A, M, K, lda, BM);
-  const CUtensorMap tb = make_tmap(B, N, K, ldb, BN);
-  GemmArgs g{};
-  g.C = C;
-  g.M = static_cast<int>(M);
-  g.N = static_cast<int>(N);
-  g.K = static_cast<int>(K);
-  g.ldc = static_cast<int>(ldc);
-  const int tiles = static_cast<int>(((M + BM - 1) / BM) * ((N + BN - 1) / BN));
-  const int grid = std::max(1, std::min(tiles, sm_count));
+  const CUtensorMap tb = make_tmap(B, N, K, ldb, tile_n<false>());
+  GemmArgs g = plain_args(C, M, N, K, ldc);
   if (mse) {
     set_mse(g, mse);
-    launch<false, 1, false>(grid, ta, tb, g, CommArgs{}, stream, "gemm_mse_epilogue");
+    launch<false, kMse, false>(sm_count, ta, tb, g, stream, "gemm_mse_epilogue");
   } else {
-    launch<false, 0, false>(grid, ta, tb, g, CommArgs{}, stream, "gemm_bf16_tn");
+    launch<false, kStore, false>(sm_count, ta, tb, g, stream, "gemm_bf16_tn");
   }
 }
 
 bool gemm_bf16_nn_supported(int64_t M, int64_t N, int64_t K, const void* A, const void* B, const void* C, int64_t lda,
                             int64_t ldb, int64_t ldc) {
-  auto al = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
-  return M > 0 && N > 0 && K > 0 && N % 8 == 0 && K % 8 == 0 && al(A) && al(B) && al(C) && lda % 8 == 0 && ldb % 8 == 0 &&
-         ldc % 8 == 0 && lda >= K && ldb >= N && ldc >= N && M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31);
+  return M > 0 && N > 0 && K > 0 && N % 8 == 0 && K % 8 == 0 && aligned16(A) && aligned16(B) && aligned16(C) &&
+         lda % 8 == 0 && ldb % 8 == 0 && ldc % 8 == 0 && lda >= K && ldb >= N && ldc >= N && M < (1ll << 31) &&
+         N < (1ll << 31) && K < (1ll << 31);
 }
 
 // C[M,N] = A[M,K] * B[K,N], both row-major (the dgrad shape: gy @ W).
 void launch_gemm_bf16_nn(const void* A, const void* B, void* C, int64_t M, int64_t N, int64_t K, int64_t lda,
                          int64_t ldb, int64_t ldc, int sm_count, cudaStream_t stream) {
   M4T_CHECK(gemm_bf16_nn_supported(M, N, K, A, B, C, lda, ldb, ldc), "unsupported GEMM shape/alignment for the wgmma NN path");
-  constexpr int BN = tile_n<false>();
   const CUtensorMap ta = make_tmap(A, M, K, lda, BM);
   const CUtensorMap tb = make_tmap_bf16_sw128(B, K, N, ldb, 64, BK);  // boxes of {64 n, BK k-rows}
-  GemmArgs g{};
-  g.C = C;
-  g.M = static_cast<int>(M);
-  g.N = static_cast<int>(N);
-  g.K = static_cast<int>(K);
-  g.ldc = static_cast<int>(ldc);
-  const int tiles = static_cast<int>(((M + BM - 1) / BM) * ((N + BN - 1) / BN));
-  const int grid = std::max(1, std::min(tiles, sm_count));
-  launch<false, 0, true>(grid, ta, tb, g, CommArgs{}, stream, "gemm_nn");
+  launch<false, kStore, true>(sm_count, ta, tb, plain_args(C, M, N, K, ldc), stream, "gemm_nn");
 }
 
 // y = x @ mean_ranks(W)^T in ONE kernel.  `w_off`/`wavg_off`/`flags_off` are
@@ -619,12 +602,7 @@ void launch_fused_allreduce_gemm(const DeviceComm& dc, const void* x, void* y, i
   constexpr int BN = tile_n<true>();
   const CUtensorMap ta = make_tmap(x, M, K, ldx, BM);
   const CUtensorMap tb = make_tmap(wavg, N, K, K, BN);
-  GemmArgs g{};
-  g.C = y;
-  g.M = static_cast<int>(M);
-  g.N = static_cast<int>(N);
-  g.K = static_cast<int>(K);
-  g.ldc = static_cast<int>(ldy);
+  GemmArgs g = plain_args(y, M, N, K, ldy);
   g.panel_flags = reinterpret_cast<const uint32_t*>(dc.heap[dc.sync.rank] + flags_off);
   g.panel_target = panel_target;
   CommArgs cm{};
@@ -643,9 +621,9 @@ void launch_fused_allreduce_gemm(const DeviceComm& dc, const void* x, void* y, i
   const int grid = fused_gemm_grid(dc);
   if (mse) {
     set_mse(g, mse);
-    launch<true, 1, false>(grid, ta, tb, g, cm, stream, "fused_allreduce_gemm_mse");
+    launch<true, kMse, false>(grid, ta, tb, g, stream, "fused_allreduce_gemm_mse", MlpEpiArgs{}, cm);
   } else {
-    launch<true, 0, false>(grid, ta, tb, g, cm, stream, "fused_allreduce_gemm");
+    launch<true, kStore, false>(grid, ta, tb, g, stream, "fused_allreduce_gemm", MlpEpiArgs{}, cm);
   }
 }
 
@@ -653,14 +631,14 @@ int64_t colsum_rows(int64_t M) { return (M + 15) / 16; }
 
 void launch_gemm_bias_gelu(const void* A, const void* B, const float* bias, void* z, void* h, int64_t M, int64_t N,
                            int64_t K, int64_t lda, int64_t ldb, int64_t ldc, int sm_count, cudaStream_t stream) {
-  M4T_CHECK(gemm_bf16_tn_supported(M, N, K, A, B, z, lda, ldb, ldc) && (reinterpret_cast<uintptr_t>(h) & 15u) == 0,
+  M4T_CHECK(gemm_bf16_tn_supported(M, N, K, A, B, z, lda, ldb, ldc) && aligned16(h),
             "unsupported GEMM shape/alignment for the wgmma bias+GELU path");
   M4T_CHECK(epilogue_bias_ok(bias), "the bias needs an 8-byte-aligned base");
   MlpEpiArgs e{};
   e.bias = bias;
   e.h_out = h;
-  launch<false, 2, false>(plain_grid(M, N, sm_count), make_tmap(A, M, K, lda, BM), make_tmap(B, N, K, ldb, tile_n<false>()),
-                          plain_args(z, M, N, K, ldc), CommArgs{}, stream, "gemm_bias_gelu", e);
+  launch<false, kBiasGelu, false>(sm_count, make_tmap(A, M, K, lda, BM), make_tmap(B, N, K, ldb, tile_n<false>()),
+                           plain_args(z, M, N, K, ldc), stream, "gemm_bias_gelu", e);
 }
 
 void launch_gemm_bias_mse_colsum(const void* A, const void* B, const float* bias, void* dy, float* colsum, int64_t M,
@@ -674,8 +652,8 @@ void launch_gemm_bias_mse_colsum(const void* A, const void* B, const float* bias
   MlpEpiArgs e{};
   e.bias = bias;
   e.colsum = colsum;
-  launch<false, 3, false>(plain_grid(M, N, sm_count), make_tmap(A, M, K, lda, BM), make_tmap(B, N, K, ldb, tile_n<false>()),
-                          g, CommArgs{}, stream, "gemm_bias_mse_colsum", e);
+  launch<false, kBiasMseColsum, false>(sm_count, make_tmap(A, M, K, lda, BM), make_tmap(B, N, K, ldb, tile_n<false>()), g,
+                                stream, "gemm_bias_mse_colsum", e);
 }
 
 void launch_gemm_nn_gelu_bwd_colsum(const void* A, const void* B, const void* z, void* dz, float* colsum, int64_t M,
@@ -690,17 +668,14 @@ void launch_gemm_nn_gelu_bwd_colsum(const void* A, const void* B, const void* z,
   MlpEpiArgs e{};
   e.colsum = colsum;
   e.gscale = gscale;
-  launch<false, 4, true>(plain_grid(M, N, sm_count), make_tmap(A, M, K, lda, BM), make_tmap_bf16_sw128(B, K, N, ldb, 64, BK),
-                         g, CommArgs{}, stream, "gemm_nn_gelu_bwd_colsum", e);
+  launch<false, kGeluBwdColsum, true>(sm_count, make_tmap(A, M, K, lda, BM), make_tmap_bf16_sw128(B, K, N, ldb, 64, BK), g,
+                               stream, "gemm_nn_gelu_bwd_colsum", e);
 }
 
 void launch_column_sum(const float* partial, int64_t rows, int64_t N, float* out, const float* gscale, cudaStream_t stream) {
   M4T_CHECK(rows > 0 && N > 0 && N < (1ll << 31) && rows < (1ll << 31), "column_sum: empty or oversized workspace");
-  column_sum_kernel<<<static_cast<unsigned>((N + 31) / 32), 256, 0, stream>>>(partial, static_cast<int>(rows),
-                                                                              static_cast<int>(N), out, gscale);
-  cudaError_t err = cudaGetLastError();
-  M4T_CHECK(err == cudaSuccess, "column_sum launch failed: " << cudaGetErrorString(err));
-  note_kernel_launch("column_sum");
+  launch_kernel<column_sum_kernel<>>(static_cast<unsigned>((N + 31) / 32), 256, 0, stream, "column_sum", partial,
+                                     static_cast<int>(rows), static_cast<int>(N), out, gscale);
 }
 
 int64_t xent_tiles(int64_t N) { return (N + tile_n<false>() - 1) / tile_n<false>(); }
@@ -713,24 +688,22 @@ void launch_gemm_bias_xent(const void* A, const void* B, const float* bias, void
   MlpEpiArgs e{};
   e.bias = bias;
   e.xent_ms = ms;
-  launch<false, 5, false>(plain_grid(M, N, sm_count), make_tmap(A, M, K, lda, BM), make_tmap(B, N, K, ldb, tile_n<false>()),
-                          plain_args(logits, M, N, K, ldc), CommArgs{}, stream, "gemm_bias_xent", e);
+  launch<false, kBiasXent, false>(sm_count, make_tmap(A, M, K, lda, BM), make_tmap(B, N, K, ldb, tile_n<false>()),
+                           plain_args(logits, M, N, K, ldc), stream, "gemm_bias_xent", e);
 }
 
 void launch_xent_finish(void* y, int64_t M, int64_t N, int64_t ldy, const float2* ms, const int64_t* labels,
                         int64_t ignore_index, float loss_scale, float grad_scale, float* row_loss, unsigned int* done,
                         float* loss, float* colsum, cudaStream_t stream) {
-  M4T_CHECK(M > 0 && N > 0 && N % 8 == 0 && ldy % 8 == 0 && ldy >= N && (reinterpret_cast<uintptr_t>(y) & 15u) == 0 &&
-                (reinterpret_cast<uintptr_t>(colsum) & 15u) == 0 && M < (1ll << 31) && N < (1ll << 31),
+  M4T_CHECK(M > 0 && N > 0 && N % 8 == 0 && ldy % 8 == 0 && ldy >= N && aligned16(y) && aligned16(colsum) &&
+                M < (1ll << 31) && N < (1ll << 31),
             "xent_finish: unsupported shape or alignment");
   const int64_t blocks = ((M + kXentRows - 1) / kXentRows) * ((N + kXentCols - 1) / kXentCols);
   M4T_CHECK(blocks < (1ll << 31), "xent_finish: too many blocks");
-  xent_finish_kernel<<<static_cast<unsigned>(blocks), kXentThreads, 0, stream>>>(
-      static_cast<uint16_t*>(y), ldy, ms, static_cast<int>(xent_tiles(N)), labels, static_cast<int>(M), static_cast<int>(N),
-      ignore_index, loss_scale, grad_scale, row_loss, done, loss, colsum);
-  cudaError_t err = cudaGetLastError();
-  M4T_CHECK(err == cudaSuccess, "xent_finish launch failed: " << cudaGetErrorString(err));
-  note_kernel_launch("xent_finish");
+  launch_kernel<xent_finish_kernel>(static_cast<unsigned>(blocks), kXentThreads, 0, stream, "xent_finish",
+                                    static_cast<uint16_t*>(y), ldy, ms, static_cast<int>(xent_tiles(N)), labels,
+                                    static_cast<int>(M), static_cast<int>(N), ignore_index, loss_scale, grad_scale,
+                                    row_loss, done, loss, colsum);
 }
 
 int fused_gemm_grid(const DeviceComm& dc) { return std::min(dc.sm_count, kMaxChannels) & ~1; }
@@ -739,32 +712,19 @@ int fused_gemm_grid(const DeviceComm& dc) { return std::min(dc.sm_count, kMaxCha
 // Every operand is contiguous and stacked along its leading dimension, so expert e's A rows are rows [e M, e M + M) of
 // one [E M, K] matrix and the whole call is ONE GEMM of E M rows against a B that changes at every M rows.
 bool batched_gemm_supported(int64_t E, int64_t M, int64_t N, int64_t K, const void* A, const void* B, const void* C) {
-  auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
-  return E > 0 && M > 0 && N > 0 && K > 0 && M % BM == 0 && N % 128 == 0 && K % 128 == 0 && al16(A) && al16(B) &&
-         al16(C) && E * M < (1ll << 31) && E * N < (1ll << 31) && E * K < (1ll << 31);
+  return E > 0 && M > 0 && N > 0 && K > 0 && M % BM == 0 && N % 128 == 0 && K % 128 == 0 && aligned16(A) &&
+         aligned16(B) && aligned16(C) && E * M < (1ll << 31) && E * N < (1ll << 31) && E * K < (1ll << 31);
 }
-
-namespace {
-
-GemmArgs batched_args(void* C, int64_t E, int64_t M, int64_t N, int64_t K) {
-  GemmArgs g = plain_args(C, E * M, N, K, N);
-  g.expert_rows = static_cast<int>(M);
-  return g;
-}
-
-}  // namespace
 
 void launch_gemm_bias_gelu_batched(const void* A, const void* B, const float* bias, void* z, void* h, int64_t E,
                                    int64_t M, int64_t N, int64_t K, int sm_count, cudaStream_t stream) {
-  M4T_CHECK(batched_gemm_supported(E, M, N, K, A, B, z) && (reinterpret_cast<uintptr_t>(h) & 15u) == 0 &&
-                epilogue_bias_ok(bias),
+  M4T_CHECK(batched_gemm_supported(E, M, N, K, A, B, z) && aligned16(h) && epilogue_bias_ok(bias),
             "unsupported shape/alignment for the batched bias+GELU GEMM");
   MlpEpiArgs e{};
   e.bias = bias;
   e.h_out = h;
-  launch<false, 2, false, true>(plain_grid(E * M, N, sm_count), make_tmap(A, E * M, K, K, BM),
-                                make_tmap(B, E * N, K, K, tile_n<false>()), batched_args(z, E, M, N, K), CommArgs{},
-                                stream, "gemm_bias_gelu_batched", e);
+  launch<false, kBiasGelu, false, true>(sm_count, make_tmap(A, E * M, K, K, BM), make_tmap(B, E * N, K, K, tile_n<false>()),
+                                 batched_args(z, E, M, N, K), stream, "gemm_bias_gelu_batched", e);
 }
 
 void launch_gemm_bias_batched(const void* A, const void* B, const float* bias, void* y, int64_t E, int64_t M, int64_t N,
@@ -773,9 +733,8 @@ void launch_gemm_bias_batched(const void* A, const void* B, const float* bias, v
             "unsupported shape/alignment for the batched bias GEMM");
   MlpEpiArgs e{};
   e.bias = bias;
-  launch<false, 6, false, true>(plain_grid(E * M, N, sm_count), make_tmap(A, E * M, K, K, BM),
-                                make_tmap(B, E * N, K, K, tile_n<false>()), batched_args(y, E, M, N, K), CommArgs{},
-                                stream, "gemm_bias_batched", e);
+  launch<false, kBias, false, true>(sm_count, make_tmap(A, E * M, K, K, BM), make_tmap(B, E * N, K, K, tile_n<false>()),
+                             batched_args(y, E, M, N, K), stream, "gemm_bias_batched", e);
 }
 
 void launch_gemm_nn_gelu_bwd_colsum_batched(const void* A, const void* B, const void* z, void* dz, float* colsum,
@@ -789,17 +748,15 @@ void launch_gemm_nn_gelu_bwd_colsum_batched(const void* A, const void* B, const 
   MlpEpiArgs e{};
   e.colsum = colsum;
   e.gscale = gscale;
-  launch<false, 4, true, true>(plain_grid(E * M, N, sm_count), make_tmap(A, E * M, K, K, BM),
-                               make_tmap_bf16_sw128(B, E * K, N, N, 64, BK), g, CommArgs{}, stream,
-                               "gemm_nn_gelu_bwd_colsum_batched", e);
+  launch<false, kGeluBwdColsum, true, true>(sm_count, make_tmap(A, E * M, K, K, BM), make_tmap_bf16_sw128(B, E * K, N, N, 64, BK),
+                                     g, stream, "gemm_nn_gelu_bwd_colsum_batched", e);
 }
 
 void launch_gemm_nn_batched(const void* A, const void* B, void* C, int64_t E, int64_t M, int64_t N, int64_t K,
                             int sm_count, cudaStream_t stream) {
   M4T_CHECK(batched_gemm_supported(E, M, N, K, A, B, C), "unsupported shape/alignment for the batched NN GEMM");
-  launch<false, 0, true, true>(plain_grid(E * M, N, sm_count), make_tmap(A, E * M, K, K, BM),
-                               make_tmap_bf16_sw128(B, E * K, N, N, 64, BK), batched_args(C, E, M, N, K), CommArgs{},
-                               stream, "gemm_nn_batched");
+  launch<false, kStore, true, true>(sm_count, make_tmap(A, E * M, K, K, BM), make_tmap_bf16_sw128(B, E * K, N, N, 64, BK),
+                             batched_args(C, E, M, N, K), stream, "gemm_nn_batched");
 }
 
 void launch_column_sum_batched(const float* partial, int64_t E, int64_t rows, int64_t N, float* out, const float* gscale,
@@ -807,10 +764,8 @@ void launch_column_sum_batched(const float* partial, int64_t E, int64_t rows, in
   M4T_CHECK(E > 0 && E < 65536 && rows > 0 && N > 0 && N < (1ll << 31) && rows * N < (1ll << 31),
             "column_sum_batched: empty or oversized workspace");
   const dim3 grid(static_cast<unsigned>((N + 31) / 32), static_cast<unsigned>(E));
-  column_sum_kernel<true><<<grid, 256, 0, stream>>>(partial, static_cast<int>(rows), static_cast<int>(N), out, gscale);
-  cudaError_t err = cudaGetLastError();
-  M4T_CHECK(err == cudaSuccess, "column_sum_batched launch failed: " << cudaGetErrorString(err));
-  note_kernel_launch("column_sum_batched");
+  launch_kernel<column_sum_kernel<true>>(grid, 256, 0, stream, "column_sum_batched", partial, static_cast<int>(rows),
+                                         static_cast<int>(N), out, gscale);
 }
 
 }  // namespace m4t

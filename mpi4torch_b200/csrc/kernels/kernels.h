@@ -177,8 +177,6 @@ void launch_wgrad_bf16(const void* dy, const void* x, void* g, int64_t Mb, int64
 // (the single-rank SGD step as the GEMM's own epilogue).
 // acc[N,K] (contiguous fp32) <- fmaf(gscale, dy^T x, acc) elementwise: one rounding per call.  Gradient
 // accumulation over micro-batches; the operand rules are wgrad_bf16_supported's with ldg = K.
-bool wgrad_accumulate_supported(int64_t Mb, int64_t N, int64_t K, const void* dy, const void* x, const float* acc,
-                                int64_t ldy, int64_t ldx);
 void launch_wgrad_accumulate(const void* dy, const void* x, float* acc, int64_t Mb, int64_t N, int64_t K, int64_t ldy,
                              int64_t ldx, int sm_count, cudaStream_t stream, const float* gscale = nullptr);
 // wgrad GEMM -> reduce-scatter through the switch -> W += scale * sum -> multicast of the new

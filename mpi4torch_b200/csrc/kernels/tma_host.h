@@ -1,13 +1,43 @@
-// Host-side construction of TMA descriptors (CUtensorMap) for row-major bf16 matrices.
+// Host side of the GEMM kernels (gemm_wgmma.cu, wgrad_wgmma.cu, gemm_fp8.cu): TMA descriptors (CUtensorMap) for
+// row-major bf16 and fp8 matrices, the operand alignment test, the persistent grid and the checked launch.
 // cuTensorMapEncodeTiled is resolved through the runtime (cudaGetDriverEntryPoint), so the
 // extension does not link libcuda.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 
+#include <algorithm>
+#include <mutex>
+
 #include "../runtime/common.h"
+#include "kernels.h"
 
 namespace m4t {
+
+// TMA bases and the epilogues' 16-byte vector accesses need 16-byte-aligned addresses.
+inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+
+// One persistent CTA per SM, never more CTAs than tiles, and at least one.
+inline int persistent_grid(int64_t tiles, int sm_count) {
+  return static_cast<int>(std::max<int64_t>(1, std::min<int64_t>(tiles, sm_count)));
+}
+
+// Launches Kernel<<<grid, threads, smem, stream>>>(args...), checks the launch and counts it under `what`.  A kernel
+// with dynamic shared memory (smem > 0; always the same amount for one kernel) gets its limit raised on first use.
+template <auto Kernel, typename... Args>
+void launch_kernel(dim3 grid, int threads, int smem, cudaStream_t stream, const char* what, const Args&... args) {
+  if (smem > 0) {
+    static std::once_flag once;
+    std::call_once(once, [smem] {
+      const cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+      M4T_CHECK(e == cudaSuccess, "cudaFuncSetAttribute(smem) failed: " << cudaGetErrorString(e));
+    });
+  }
+  Kernel<<<grid, threads, smem, stream>>>(args...);
+  const cudaError_t err = cudaGetLastError();
+  M4T_CHECK(err == cudaSuccess, what << " launch failed: " << cudaGetErrorString(err));
+  note_kernel_launch(what);
+}
 
 inline CUresult encode_tiled_2d(CUtensorMap* map, CUtensorMapDataType dt, void* base, const cuuint64_t* dims,
                                 const cuuint64_t* strides, const cuuint32_t* box, CUtensorMapSwizzle swizzle) {

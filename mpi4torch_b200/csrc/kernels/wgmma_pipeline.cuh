@@ -1,7 +1,7 @@
 // Shared main loop of the Hopper GEMM kernels (gemm_wgmma.cu, wgrad_wgmma.cu).
 //
-// One persistent CTA per SM computes 128 x BN output tiles (BN = 256, or 128 for the fused
-// kernels, whose communication warps need the registers) with BK = 64:
+// One persistent CTA per SM computes 128 x BN output tiles (BN = tile_n<FUSED>(): 256, or 128 for
+// the fused kernels, whose communication warps need the registers) with BK = 64:
 //   warpgroup 0 (warp 0, one lane)  TMA producer: A/B tiles -> smem ring of Tile<BN>::kStages
 //   warpgroups 1, 2                 consumers: 64 rows each, wgmma m64nBNk16 into BN/2 fp32
 //                                   registers per thread, epilogue straight from registers
@@ -30,6 +30,12 @@ template <int BN> struct Tile {
   static constexpr int kStages = BN == 256 ? 4 : kMaxStages;  // ~192 KiB of ring either way
   static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align*/ + 256 /*barriers*/;
 };
+
+// The fused kernels' communication warps need registers: half-width tiles there.
+template <bool FUSED> constexpr int tile_n() { return FUSED ? 128 : 256; }
+// Communication warps of a fused kernel.  The wgrad owner role keeps its rows in registers, so its in-flight round
+// trips scale with warps x rows.
+constexpr int kCommWarps = 4;
 
 struct __align__(8) Pipe {
   uint64_t full[kMaxStages];

@@ -29,9 +29,7 @@
 //     rank's weights are final.
 #include <cuda.h>
 
-#include <algorithm>
 #include <atomic>
-#include <mutex>
 
 #include "kernels.h"
 #include "tma_host.h"
@@ -43,11 +41,8 @@ namespace {
 
 using namespace wg;
 
-constexpr int kCommWarps = 4;       // owner role: in-flight round trips scale with warps x rows (registers hold the data)
 constexpr int kSignalsPerUnit = kConsumerWarps;  // every consumer warp of the CTA arrives on the tile counter
 constexpr int kMaxUnicastRanks = 3;  // peer-load mode keeps ranks x rows x partial buffers requests in registers
-// the fused kernel's owner warps need registers: half-width tiles there (the plain kernel's last tile may be half)
-template <bool FUSED> constexpr int tile_n() { return FUSED ? 128 : 256; }
 
 struct WgradArgs {
   void* out;            // plain: G [N, K] (bf16; fp32 when ACC32); fused: unused (the staging buffers live in
@@ -296,6 +291,64 @@ __device__ __forceinline__ void comm_reduce_update(const WgradComm& wc, int firs
   asm volatile("bar.sync 1, %0;" ::"n"(kCommThreads));
 }
 
+// Epilogues of one consumer warpgroup's 64 rows of the tile (n_blk, k_blk) of out (leading dimension ldo, K columns).
+// The tile's columns are a multiple of 128: a last tile of K may be half.
+// bf16 out <- gs * acc, or out <- out + gs * acc when axpy.
+template <int BN>
+__device__ __forceinline__ void bf16_epilogue(const float (&acc)[BN / 2], char* obase, int ldo, int K, float gs, bool axpy,
+                                              int n_blk, int k_blk, int wgi) {
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int row = n_blk * BM + wgi * 64 + frag_row(hr);
+    uint16_t* orow = reinterpret_cast<uint16_t*>(obase) + static_cast<int64_t>(row) * ldo + k_blk * BN;
+    const int cols = min(BN, K - k_blk * BN);
+#pragma unroll
+    for (int j0 = 0; j0 < BN / 8; j0 += 8) {
+      if (j0 * 8 >= cols) continue;
+      uint32_t prev[8];
+      if (axpy) {  // the eight pieces of the row are requested before any is consumed
+#pragma unroll
+        for (int j = 0; j < 8; ++j) prev[j] = *reinterpret_cast<const uint32_t*>(orow + frag_col(j0 + j));
+      }
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        float v0 = gs * acc[4 * (j0 + j) + 2 * hr], v1 = gs * acc[4 * (j0 + j) + 2 * hr + 1];
+        if (axpy) {
+          v0 += bf16_bits_to_float(static_cast<uint16_t>(prev[j] & 0xffffu));
+          v1 += bf16_bits_to_float(static_cast<uint16_t>(prev[j] >> 16));
+        }
+        *reinterpret_cast<uint32_t*>(orow + frag_col(j0 + j)) = pack_bf16x2(v0, v1);
+      }
+    }
+  }
+}
+
+// fp32 out <- fmaf(gs, acc, out): ONE rounding per micro-batch (the product is not rounded on its own), so a
+// contribution far below the buffer's ulp still moves it by its correctly rounded share.
+template <int BN>
+__device__ __forceinline__ void acc32_epilogue(const float (&acc)[BN / 2], char* obase, int ldo, int K, float gs,
+                                               int n_blk, int k_blk, int wgi) {
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int row = n_blk * BM + wgi * 64 + frag_row(hr);
+    float* orow = reinterpret_cast<float*>(obase) + static_cast<int64_t>(row) * ldo + k_blk * BN;
+    const int cols = min(BN, K - k_blk * BN);
+#pragma unroll
+    for (int j0 = 0; j0 < BN / 8; j0 += 8) {
+      if (j0 * 8 >= cols) continue;
+      float2 prev[8];  // the eight column pairs of the row are requested before any is consumed
+#pragma unroll
+      for (int j = 0; j < 8; ++j) prev[j] = *reinterpret_cast<const float2*>(orow + frag_col(j0 + j));
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float2 o = make_float2(fmaf(gs, acc[4 * (j0 + j) + 2 * hr], prev[j].x),
+                                     fmaf(gs, acc[4 * (j0 + j) + 2 * hr + 1], prev[j].y));
+        *reinterpret_cast<float2*>(orow + frag_col(j0 + j)) = o;
+      }
+    }
+  }
+}
+
 // ACC32 (plain mode only): out is an fp32 [N, K] buffer and the epilogue is out <- fmaf(gscale, G, out), the
 // gradient accumulation of micro-batches.  A compile-time mode, so the other instantiations are unchanged.
 // BATCHED (plain mode only): E = g.experts problems G_e = dY_e^T X_e of the same shape, with dY [E Mb, N], X [E Mb, K]
@@ -377,54 +430,8 @@ wgrad_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
       }
       const float gs = (g.gscale ? __ldg(g.gscale) : 1.0f) * (g.axpy != 0.0f ? g.axpy : 1.0f);
       const bool axpy = !FUSED && g.axpy != 0.0f;
-      if constexpr (ACC32) {
-        // out[r, c] <- fmaf(gs, acc, out[r, c]): ONE rounding per micro-batch (the product is not rounded on its
-        // own), so a contribution far below the buffer's ulp still moves it by its correctly rounded share.
-#pragma unroll
-        for (int hr = 0; hr < 2; ++hr) {
-          const int row = n_blk * BM + wgi * 64 + frag_row(hr);
-          float* orow = reinterpret_cast<float*>(obase) + static_cast<int64_t>(row) * ldo + k_blk * BN;
-          const int cols = min(BN, g.K - k_blk * BN);  // a multiple of 128
-#pragma unroll
-          for (int j0 = 0; j0 < BN / 8; j0 += 8) {
-            if (j0 * 8 >= cols) continue;
-            float2 prev[8];  // the eight column pairs of the row are requested before any is consumed
-#pragma unroll
-            for (int j = 0; j < 8; ++j) prev[j] = *reinterpret_cast<const float2*>(orow + frag_col(j0 + j));
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float2 o = make_float2(fmaf(gs, acc[4 * (j0 + j) + 2 * hr], prev[j].x),
-                                           fmaf(gs, acc[4 * (j0 + j) + 2 * hr + 1], prev[j].y));
-              *reinterpret_cast<float2*>(orow + frag_col(j0 + j)) = o;
-            }
-          }
-        }
-        continue;
-      }
-#pragma unroll
-      for (int hr = 0; hr < 2; ++hr) {
-        const int row = n_blk * BM + wgi * 64 + frag_row(hr);
-        uint16_t* orow = reinterpret_cast<uint16_t*>(obase) + static_cast<int64_t>(row) * ldo + k_blk * BN;
-        const int cols = min(BN, g.K - k_blk * BN);  // a multiple of 128
-#pragma unroll
-        for (int j0 = 0; j0 < BN / 8; j0 += 8) {
-          if (j0 * 8 >= cols) continue;
-          uint32_t prev[8];
-          if (axpy) {  // the eight pieces of the row are requested before any is consumed
-#pragma unroll
-            for (int j = 0; j < 8; ++j) prev[j] = *reinterpret_cast<const uint32_t*>(orow + frag_col(j0 + j));
-          }
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            float v0 = gs * acc[4 * (j0 + j) + 2 * hr], v1 = gs * acc[4 * (j0 + j) + 2 * hr + 1];
-            if (axpy) {
-              v0 += bf16_bits_to_float(static_cast<uint16_t>(prev[j] & 0xffffu));
-              v1 += bf16_bits_to_float(static_cast<uint16_t>(prev[j] >> 16));
-            }
-            *reinterpret_cast<uint32_t*>(orow + frag_col(j0 + j)) = pack_bf16x2(v0, v1);
-          }
-        }
-      }
+      if constexpr (ACC32) acc32_epilogue<BN>(acc, obase, ldo, g.K, gs, n_blk, k_blk, wgi);
+      else bf16_epilogue<BN>(acc, obase, ldo, g.K, gs, axpy, n_blk, k_blk, wgi);
       if (FUSED && !(wc.debug & 16)) {
         // this warp's 16 rows of the partial tile are written: tell the owner.  The release
         // (a system-scope fence + the add) is cumulative over the warp's stores through __syncwarp.
@@ -449,16 +456,20 @@ CUtensorMap make_tmap_mn(const void* base, int64_t rows, int64_t cols, int64_t l
   return make_tmap_bf16_sw128(base, rows, cols, ld, 64, BK);
 }
 
-template <bool FUSED, bool ACC32 = false, bool BATCHED = false> void configure_w() {
-  static std::once_flag once;
-  std::call_once(once, [] {
-    cudaError_t e = cudaFuncSetAttribute(wgrad_bf16_wgmma_kernel<FUSED, ACC32, BATCHED>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Tile<tile_n<FUSED>()>::kSmemBytes);
-    M4T_CHECK(e == cudaSuccess, "cudaFuncSetAttribute(smem) failed: " << cudaGetErrorString(e));
-  });
+WgradArgs wgrad_args(void* out, int64_t Mb, int64_t N, int64_t K, int64_t ldo, int ksplit, const float* gscale,
+                     float axpy, int64_t experts = 0) {
+  WgradArgs g{};
+  g.out = out;
+  g.Mb = static_cast<int>(Mb);
+  g.N = static_cast<int>(N);
+  g.K = static_cast<int>(K);
+  g.ldo = static_cast<int>(ldo);
+  g.ksplit = ksplit;
+  g.gscale = gscale;
+  g.axpy = axpy;
+  g.experts = static_cast<int>(experts);
+  return g;
 }
-
-bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 }  // namespace
 
@@ -477,55 +488,22 @@ void launch_wgrad_bf16(const void* dy, const void* x, void* gout, int64_t Mb, in
                        int64_t ldx, int64_t ldg, int sm_count, cudaStream_t stream, const float* gscale, float axpy) {
   M4T_CHECK(wgrad_bf16_supported(Mb, N, K, dy, x, gout, ldy, ldx, ldg),
             "unsupported wgrad shape/alignment for the wgmma path (N % 128, K % 128, batch % 64)");
-  const CUtensorMap ta = make_tmap_mn(dy, Mb, N, ldy);
-  const CUtensorMap tb = make_tmap_mn(x, Mb, K, ldx);
-  WgradArgs g{};
-  g.out = gout;
-  g.Mb = static_cast<int>(Mb);
-  g.N = static_cast<int>(N);
-  g.K = static_cast<int>(K);
-  g.ldo = static_cast<int>(ldg);
-  g.ksplit = 1;
-  g.gscale = gscale;
-  g.axpy = axpy;
   constexpr int BN = tile_n<false>();
-  const int tiles = static_cast<int>((N / BM) * ((K + BN - 1) / BN));
-  const int grid = std::max(1, std::min(tiles, sm_count));
-  configure_w<false>();
-  wgrad_bf16_wgmma_kernel<false><<<grid, kGemmThreads, Tile<BN>::kSmemBytes, stream>>>(ta, tb, g, WgradComm{});
-  cudaError_t e = cudaGetLastError();
-  M4T_CHECK(e == cudaSuccess, "wgrad_bf16 launch failed: " << cudaGetErrorString(e));
-  note_kernel_launch(axpy != 0.0f ? "wgrad_sgd_epilogue" : "wgrad");
-}
-
-bool wgrad_accumulate_supported(int64_t Mb, int64_t N, int64_t K, const void* dy, const void* x, const float* acc,
-                                int64_t ldy, int64_t ldx) {
-  return wgrad_bf16_supported(Mb, N, K, dy, x, acc, ldy, ldx, K);
+  launch_kernel<wgrad_bf16_wgmma_kernel<false>>(
+      persistent_grid((N / BM) * ((K + BN - 1) / BN), sm_count), kGemmThreads, Tile<BN>::kSmemBytes, stream,
+      axpy != 0.0f ? "wgrad_sgd_epilogue" : "wgrad", make_tmap_mn(dy, Mb, N, ldy), make_tmap_mn(x, Mb, K, ldx),
+      wgrad_args(gout, Mb, N, K, ldg, 1, gscale, axpy), WgradComm{});
 }
 
 void launch_wgrad_accumulate(const void* dy, const void* x, float* acc, int64_t Mb, int64_t N, int64_t K, int64_t ldy,
                              int64_t ldx, int sm_count, cudaStream_t stream, const float* gscale) {
-  M4T_CHECK(wgrad_accumulate_supported(Mb, N, K, dy, x, acc, ldy, ldx),
+  M4T_CHECK(wgrad_bf16_supported(Mb, N, K, dy, x, acc, ldy, ldx, K),
             "unsupported wgrad_accumulate shape/alignment (N % 128, K % 128, batch % 64, 16-byte aligned operands)");
-  const CUtensorMap ta = make_tmap_mn(dy, Mb, N, ldy);
-  const CUtensorMap tb = make_tmap_mn(x, Mb, K, ldx);
-  WgradArgs g{};
-  g.out = acc;
-  g.Mb = static_cast<int>(Mb);
-  g.N = static_cast<int>(N);
-  g.K = static_cast<int>(K);
-  g.ldo = static_cast<int>(K);
-  g.ksplit = 1;
-  g.gscale = gscale;
-  g.axpy = 0.0f;
   constexpr int BN = tile_n<false>();
-  const int tiles = static_cast<int>((N / BM) * ((K + BN - 1) / BN));
-  const int grid = std::max(1, std::min(tiles, sm_count));
-  configure_w<false, true>();
-  wgrad_bf16_wgmma_kernel<false, true><<<grid, kGemmThreads, Tile<BN>::kSmemBytes, stream>>>(ta, tb, g, WgradComm{});
-  cudaError_t e = cudaGetLastError();
-  M4T_CHECK(e == cudaSuccess, "wgrad_accumulate launch failed: " << cudaGetErrorString(e));
-  note_kernel_launch("wgrad_accumulate");
+  launch_kernel<wgrad_bf16_wgmma_kernel<false, true>>(
+      persistent_grid((N / BM) * ((K + BN - 1) / BN), sm_count), kGemmThreads, Tile<BN>::kSmemBytes, stream,
+      "wgrad_accumulate", make_tmap_mn(dy, Mb, N, ldy), make_tmap_mn(x, Mb, K, ldx),
+      wgrad_args(acc, Mb, N, K, K, 1, gscale, 0.0f), WgradComm{});
 }
 
 bool wgrad_bf16_batched_supported(int64_t E, int64_t Mb, int64_t N, int64_t K, const void* dy, const void* x,
@@ -538,26 +516,11 @@ void launch_wgrad_bf16_batched(const void* dy, const void* x, void* gout, int64_
                                int sm_count, cudaStream_t stream, const float* gscale) {
   M4T_CHECK(wgrad_bf16_batched_supported(E, Mb, N, K, dy, x, gout),
             "unsupported shape/alignment for the batched wgrad (N % 128, K % 128, batch % 64, 16-byte-aligned operands)");
-  const CUtensorMap ta = make_tmap_mn(dy, E * Mb, N, N);
-  const CUtensorMap tb = make_tmap_mn(x, E * Mb, K, K);
-  WgradArgs g{};
-  g.out = gout;
-  g.Mb = static_cast<int>(Mb);
-  g.N = static_cast<int>(N);
-  g.K = static_cast<int>(K);
-  g.ldo = static_cast<int>(K);
-  g.ksplit = 1;
-  g.gscale = gscale;
-  g.axpy = 0.0f;
-  g.experts = static_cast<int>(E);
   constexpr int BN = tile_n<false>();
-  const int64_t tiles = E * (N / BM) * ((K + BN - 1) / BN);
-  const int grid = static_cast<int>(std::max<int64_t>(1, std::min<int64_t>(tiles, sm_count)));
-  configure_w<false, false, true>();
-  wgrad_bf16_wgmma_kernel<false, false, true><<<grid, kGemmThreads, Tile<BN>::kSmemBytes, stream>>>(ta, tb, g, WgradComm{});
-  cudaError_t e = cudaGetLastError();
-  M4T_CHECK(e == cudaSuccess, "wgrad_bf16_batched launch failed: " << cudaGetErrorString(e));
-  note_kernel_launch("wgrad_bf16_batched");
+  launch_kernel<wgrad_bf16_wgmma_kernel<false, false, true>>(
+      persistent_grid(E * (N / BM) * ((K + BN - 1) / BN), sm_count), kGemmThreads, Tile<BN>::kSmemBytes, stream,
+      "wgrad_bf16_batched", make_tmap_mn(dy, E * Mb, N, N), make_tmap_mn(x, E * Mb, K, K),
+      wgrad_args(gout, Mb, N, K, K, 1, gscale, 0.0f, E), WgradComm{});
 }
 
 int64_t fused_wgrad_tiles(int64_t N, int64_t K) { return (N / BM) * (K / tile_n<true>()); }
@@ -578,15 +541,7 @@ void launch_fused_wgrad_update(const DeviceComm& dc, const void* dy, const void*
   M4T_CHECK(use_multicast || stage_stride == N * K * 2, "peer-store mode expects densely packed partial buffers");
   const CUtensorMap ta = make_tmap_mn(dy, Mb, N, ldy);
   const CUtensorMap tb = make_tmap_mn(x, Mb, K, ldx);
-  WgradArgs g{};
-  g.out = nullptr;
-  g.Mb = static_cast<int>(Mb);
-  g.N = static_cast<int>(N);
-  g.K = static_cast<int>(K);
-  g.ldo = static_cast<int>(K);
-  g.ksplit = ksplit;
-  g.gscale = gscale;
-  g.axpy = 0.0f;
+  const WgradArgs g = wgrad_args(nullptr, Mb, N, K, K, ksplit, gscale, 0.0f);
   WgradComm wc{};
   wc.sync = dc.sync;
   for (int p = 0; p < dc.sync.size; ++p) wc.heap[p] = dc.heap[p];
@@ -607,12 +562,9 @@ void launch_fused_wgrad_update(const DeviceComm& dc, const void* dy, const void*
   wc.unicast = use_multicast ? 0 : 1;
   wc.debug = g_wgrad_debug.load(std::memory_order_relaxed);
   const int grid = fused_gemm_grid(dc);  // identical on every rank
-  configure_w<true>();
-  wgrad_bf16_wgmma_kernel<true><<<grid, kGemmThreads + kCommWarps * 32, Tile<tile_n<true>()>::kSmemBytes, stream>>>(
-      ta, tb, g, wc);
-  cudaError_t e = cudaGetLastError();
-  M4T_CHECK(e == cudaSuccess, "fused_wgrad_update launch failed: " << cudaGetErrorString(e));
-  note_kernel_launch(wc.prefetch ? "fused_wgrad_reduce_scatter_sgd_prefetch" : "fused_wgrad_reduce_scatter_sgd");
+  launch_kernel<wgrad_bf16_wgmma_kernel<true>>(
+      grid, kGemmThreads + kCommWarps * 32, Tile<tile_n<true>()>::kSmemBytes, stream,
+      wc.prefetch ? "fused_wgrad_reduce_scatter_sgd_prefetch" : "fused_wgrad_reduce_scatter_sgd", ta, tb, g, wc);
 }
 
 }  // namespace m4t
