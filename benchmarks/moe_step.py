@@ -13,6 +13,17 @@ a separate ``torch.profiler`` run; FLOP/s from the shapes (forward 2 E M (D H + 
 name and power limit are read in the same run.
 
     python benchmarks/moe_step.py [--shapes small,large] [--out DIR]
+
+With ``--routing uniform|skewed`` it compares instead, on the same E * M routed (token, choice) pairs:
+
+* ``grouped``: the dropless ``grouped_expert_mlp`` node, every expert on exactly its pairs;
+* ``batched``: ``expert_mlp`` with the capacity of the largest count (rounded up to 128), so neither arm drops a pair;
+* ``grouped_mm``: eager bf16 on ``torch._grouped_mm`` with autograd, where this torch has it.
+
+Uniform routing gives every expert M pairs.  Skewed routing is seeded: expert 0 takes ``--skew`` (default 4) times the
+mean load and the others share the rest at random.  FLOP/s count the routed rows only.
+
+    python benchmarks/moe_step.py --routing skewed [--shapes small,large]
 """
 import argparse
 import json
@@ -28,7 +39,9 @@ sys.path.insert(0, ROOT)
 import mpi4torch_b200 as m4t  # noqa: E402
 from benchmarks.fp8_linear_step import kernel_times  # noqa: E402
 from benchmarks.mlp_step import card, time_ms  # noqa: E402
-from mpi4torch_b200.ops import expert_mlp, expert_mlp_supported  # noqa: E402
+from mpi4torch_b200.ops import (expert_group_starts, expert_mlp, expert_mlp_supported, grouped_expert_mlp,  # noqa: E402
+                                 grouped_expert_mlp_supported)
+from mpi4torch_b200.ops.expert_mlp import grouped_rows  # noqa: E402
 
 SHAPES = {"small": (8, 256, 1024, 4096), "large": (8, 1024, 4096, 16384)}  # E, M, D, H (O = D)
 
@@ -81,6 +94,101 @@ def make_arms(E, M, D, H):
     return {"batched": batched, "loop": loop, "eager": eager}, clear
 
 
+def route_counts(E, M, routing, skew):
+    """[E] pair counts summing to E * M: uniform, or expert 0 at skew x the mean and a seeded split of the rest."""
+    if routing == "uniform":
+        return [M] * E
+    g = torch.Generator().manual_seed(7)
+    top = int(skew * M)
+    rest = torch.multinomial(torch.ones(E - 1), E * M - top, replacement=True, generator=g)
+    counts = [top] + torch.bincount(rest, minlength=E - 1).tolist()
+    assert max(counts) == top and sum(counts) == E * M
+    return counts
+
+
+def make_routing_arms(E, M, D, H, counts):
+    g = torch.Generator(device="cuda").manual_seed(0)
+    r = lambda *s, scale=1.0: (torch.randn(*s, generator=g, device="cuda") * scale)  # noqa: E731
+    w1, w2 = r(E, H, D, scale=D ** -0.5).to(torch.bfloat16), r(E, D, H, scale=H ** -0.5).to(torch.bfloat16)
+    b1, b2 = r(E, H, scale=0.1), r(E, D, scale=0.1)
+    cnt = torch.tensor(counts, dtype=torch.int32, device="cuda")
+    starts = expert_group_starts(cnt).tolist()
+    R = grouped_rows(E * M, E)
+    xg, dyg = torch.zeros(R, D, device="cuda", dtype=torch.bfloat16), torch.zeros(R, D, device="cuda", dtype=torch.bfloat16)
+    C = -(-max(counts) // 128) * 128
+    xb, dyb = (torch.zeros(E, C, D, device="cuda", dtype=torch.bfloat16) for _ in range(2))
+    xd, dyd = r(E * M, D).to(torch.bfloat16), r(E * M, D).to(torch.bfloat16)  # dense, for torch._grouped_mm
+    at = 0
+    for e, c in enumerate(counts):
+        xg[starts[e]:starts[e] + c], dyg[starts[e]:starts[e] + c] = xd[at:at + c], dyd[at:at + c]
+        xb[e, :c], dyb[e, :c] = xd[at:at + c], dyd[at:at + c]
+        at += c
+    pg = [t.requires_grad_() for t in (xg, w1.clone(), b1.clone(), w2.clone(), b2.clone())]
+    pb = [t.requires_grad_() for t in (xb, w1.clone(), b1.clone(), w2.clone(), b2.clone())]
+    assert grouped_expert_mlp_supported(pg[0], cnt, *pg[1:]) and expert_mlp_supported(*pb)
+
+    def grouped():
+        grouped_expert_mlp(pg[0], cnt, *pg[1:]).backward(dyg)
+
+    def batched():
+        expert_mlp(*pb).backward(dyb)
+
+    arms = {"grouped": grouped, "batched": batched}
+    pe = [t.detach().clone().requires_grad_() for t in (xd, w1, w2)]
+    be = [t.to(torch.bfloat16).requires_grad_() for t in (b1, b2)]
+    offs = torch.cumsum(cnt, 0, dtype=torch.int32)
+    rows_of = torch.repeat_interleave(torch.arange(E, device="cuda"), cnt.long())
+    note = None
+    if hasattr(torch, "_grouped_mm"):
+        def grouped_mm():
+            x, w1e, w2e = pe
+            h = F.gelu(torch._grouped_mm(x, w1e.transpose(1, 2), offs=offs) + be[0][rows_of], approximate="tanh")
+            y = torch._grouped_mm(h, w2e.transpose(1, 2), offs=offs) + be[1][rows_of]
+            y.backward(dyd)
+        try:
+            grouped_mm()
+            torch.cuda.synchronize()
+            arms["grouped_mm"] = grouped_mm
+        except RuntimeError as err:  # this torch build has no kernel for it here
+            note = f"torch._grouped_mm unavailable: {str(err).splitlines()[0][:200]}"
+    else:
+        note = "torch._grouped_mm is not in this torch"
+
+    def clear():
+        for t in pg + pb + pe + be:
+            t.grad = None
+
+    return arms, clear, {"capacity_batched": C, "rows_grouped": R, "note": note}
+
+
+def routing_main(a):
+    for tag in a.shapes.split(","):
+        E, M, D, H = SHAPES[tag]
+        counts = route_counts(E, M, a.routing, a.skew)
+        arms, clear, info = make_routing_arms(E, M, D, H, counts)
+        res = {"card": card(), "routing": a.routing, "shape": {"E": E, "M_mean": M, "D": D, "H": H, "O": D},
+               "counts": counts, "max_over_mean": max(counts) / M, **info}
+        for fn in arms.values():
+            for _ in range(a.warmup):
+                fn()
+                clear()
+        torch.cuda.synchronize()
+        times = {k: [] for k in arms}
+        names = list(arms)
+        for rep in range(a.reps):
+            for k in (names if rep % 2 == 0 else names[::-1]):
+                times[k].append(time_ms(lambda k=k: (arms[k](), clear()), a.steps))
+        flops = 3 * 2.0 * E * M * (D * H + H * D)  # routed rows only
+        res["step_ms"] = {k: {"min": round(min(v), 4), "median": round(statistics.median(v), 4), "max": round(max(v), 4)}
+                          for k, v in times.items()}
+        for k in arms:
+            kt = kernel_times(lambda k=k: (arms[k](), clear()), 10, None, k)
+            total = sum(kt.values())
+            res[f"device_ms_{k}"] = round(total, 4)
+            res[f"device_tflops_{k}"] = round(flops / (total * 1e-3) / 1e12, 1)
+        print(json.dumps(res), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--shapes", default="small,large")
@@ -88,10 +196,16 @@ def main():
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--reps", type=int, default=6)
     ap.add_argument("--out", default=None, help="directory for the profiler traces")
+    ap.add_argument("--routing", choices=("uniform", "skewed"), default=None,
+                    help="compare the grouped (dropless) node with the batched one under this routing")
+    ap.add_argument("--skew", type=float, default=4.0, help="skewed routing: max / mean load")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("moe_step.py measures on the GPU; none is visible")
     assert m4t.COMM_WORLD.size == 1 and m4t.cuda_backend_ready()
+    if a.routing:
+        routing_main(a)
+        return
     if a.out:
         os.makedirs(a.out, exist_ok=True)
     for tag in a.shapes.split(","):

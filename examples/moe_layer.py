@@ -5,10 +5,12 @@ ranks), the experts are owned by their rank.  Each step prints the global loss a
 
     python -m mpi4torch_b200.launch -np 2 examples/moe_layer.py --device cpu
     python -m mpi4torch_b200.launch -np 8 examples/moe_layer.py --d-model 1024 --hidden 4096 --capacity 32
+    python -m mpi4torch_b200.launch -np 2 examples/moe_layer.py --device cpu --dropless
 
 On CUDA the experts run on the batched kernels when d_model and hidden are multiples of 128 and
 size * capacity is a multiple of 128 (the default capacity is the smallest such one); otherwise they run the torch
-composition.
+composition.  With --dropless no pair is dropped: every expert takes exactly the rows routed to it, on the grouped
+kernels when d_model and hidden are multiples of 128.
 """
 import argparse
 import math
@@ -28,6 +30,7 @@ def main() -> None:
     ap.add_argument("--hidden", type=int, default=256)
     ap.add_argument("--experts-per-rank", type=int, default=4)
     ap.add_argument("--capacity", type=int, default=0, help="0: the smallest C with size * C % 128 == 0")
+    ap.add_argument("--dropless", action="store_true", help="route without a capacity: no pair is dropped")
     ap.add_argument("--top-k", type=int, default=2)
     ap.add_argument("--lr", type=float, default=0.5)
     ap.add_argument("--device", default="cuda" if torch.cuda.is_available() else "cpu")
@@ -37,7 +40,7 @@ def main() -> None:
     cuda = args.device == "cuda"
     device = torch.device("cuda", torch.cuda.current_device()) if cuda else torch.device("cpu")
     dtype = torch.bfloat16 if cuda else torch.float32
-    capacity = args.capacity or 128 // math.gcd(128, P)
+    capacity = None if args.dropless else args.capacity or 128 // math.gcd(128, P)
     moe = ExpertParallelMLP(args.d_model, args.hidden, args.experts_per_rank, capacity, comm, top_k=args.top_k,
                             dtype=dtype, device=device, seed=3)
     head = (torch.randn(1, args.d_model, generator=torch.Generator().manual_seed(4)) / math.sqrt(args.d_model))

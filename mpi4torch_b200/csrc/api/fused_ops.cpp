@@ -556,6 +556,138 @@ Tensor batched_column_sum(const Tensor& partials, const c10::optional<Tensor>& g
   return out;
 }
 
+// ---- grouped experts (E experts with device-resident row counts, one launch per op) ------------------------------
+// x [R, K] holds expert e's rows at row 128 * sum_{j<e} ceil(counts[j] / 128) (ops.expert_group_starts); counts [E] is
+// contiguous int32 on x's device and is never read on the host.  Weights and biases are stacked as for the batched ops.
+bool bf16_2d(const Tensor& t) {
+  return t.is_cuda() && t.dim() == 2 && t.scalar_type() == at::kBFloat16 && t.is_contiguous();
+}
+
+bool counts_ok(const Tensor& counts, const Tensor& like) {
+  return counts.is_cuda() && counts.device() == like.device() && counts.dim() == 1 && counts.scalar_type() == at::kInt &&
+         counts.is_contiguous() && counts.numel() > 0;
+}
+
+// x [R, K] @ w [E, N, K]^T by groups, and the bias [E, N] (contiguous fp32, 8-byte aligned) when given.
+bool grouped_gemm_tn_ok(const Tensor& x, const Tensor& w, const Tensor& counts, const c10::optional<Tensor>& bias) {
+  if (!(bf16_2d(x) && bf16_3d(w) && same_device({&x, &w}) && counts_ok(counts, x) && counts.size(0) == w.size(0) &&
+        x.size(1) == w.size(2)))
+    return false;
+  if (bias.has_value() && !(bias->is_cuda() && bias->device() == x.device() && bias->dim() == 2 &&
+                            bias->scalar_type() == at::kFloat && bias->is_contiguous() && bias->size(0) == w.size(0) &&
+                            bias->size(1) == w.size(1) && epilogue_bias_ok(bias->data_ptr<float>())))
+    return false;
+  return World::instance().cuda_ready() && grouped_gemm_supported(w.size(0), x.size(0), w.size(1), x.size(1), x.data_ptr(),
+                                                                  w.data_ptr(), x.data_ptr(), counts.data_ptr());
+}
+
+// a [R, K] @ b [E, K, N] by groups.
+bool grouped_gemm_nn_ok(const Tensor& a, const Tensor& b, const Tensor& counts) {
+  if (!(bf16_2d(a) && bf16_3d(b) && same_device({&a, &b}) && counts_ok(counts, a) && counts.size(0) == b.size(0) &&
+        a.size(1) == b.size(1)))
+    return false;
+  return World::instance().cuda_ready() && grouped_gemm_supported(b.size(0), a.size(0), b.size(2), a.size(1), a.data_ptr(),
+                                                                  b.data_ptr(), a.data_ptr(), counts.data_ptr());
+}
+
+// dy [R, N]^T @ x [R, K] over each group's rows.
+bool grouped_wgrad_bf16_ok(const Tensor& dy, const Tensor& x, const Tensor& counts) {
+  if (!(bf16_2d(dy) && bf16_2d(x) && same_device({&dy, &x}) && counts_ok(counts, x) && dy.size(0) == x.size(0)))
+    return false;
+  return World::instance().cuda_ready() && wgrad_bf16_grouped_supported(counts.size(0), dy.size(0), dy.size(1), x.size(1),
+                                                                        dy.data_ptr(), x.data_ptr(), x.data_ptr(),
+                                                                        counts.data_ptr());
+}
+
+const char* kGroupedRules = " on one CUDA device with contiguous int32 counts [E], 1 <= E <= 1024, R % 128 == N % 128 == "
+                            "K % 128 == 0, and aligned bases";
+
+// (h, z) [R, N]: z = x_e @ w_e^T + b_e on group e's rows, h = gelu_tanh(z); other rows zero.  One launch.
+std::tuple<Tensor, Tensor> grouped_linear_bias_gelu_forward(const Tensor& x, const Tensor& w, const Tensor& b,
+                                                            const Tensor& counts) {
+  TORCH_CHECK(grouped_gemm_tn_ok(x, w, counts, b),
+              "mpi4torch_b200: grouped_linear_bias_gelu_forward needs contiguous bf16 x [R, K], w [E, N, K] and fp32 "
+              "b [E, N]", kGroupedRules);
+  c10::cuda::CUDAGuard guard(x.device());
+  Tensor z = at::empty({x.size(0), w.size(1)}, x.options());
+  Tensor h = at::empty_like(z);
+  std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
+  launch_gemm_bias_gelu_grouped(x.data_ptr(), w.data_ptr(), b.data_ptr<float>(), z.data_ptr(), h.data_ptr(),
+                                counts.data_ptr<int>(), w.size(0), x.size(0), w.size(1), x.size(1), sm_count(), stream_of(x));
+  return {h, z};
+}
+
+// y [R, N] = bf16(x_e @ w_e^T + b_e) on group e's rows, other rows zero.  One launch.
+Tensor grouped_linear_bias_forward(const Tensor& x, const Tensor& w, const Tensor& b, const Tensor& counts) {
+  TORCH_CHECK(grouped_gemm_tn_ok(x, w, counts, b),
+              "mpi4torch_b200: grouped_linear_bias_forward needs contiguous bf16 x [R, K], w [E, N, K] and fp32 b [E, N]",
+              kGroupedRules);
+  c10::cuda::CUDAGuard guard(x.device());
+  Tensor y = at::empty({x.size(0), w.size(1)}, x.options());
+  std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
+  launch_gemm_bias_grouped(x.data_ptr(), w.data_ptr(), b.data_ptr<float>(), y.data_ptr(), counts.data_ptr<int>(),
+                           w.size(0), x.size(0), w.size(1), x.size(1), sm_count(), stream_of(x));
+  return y;
+}
+
+// (dz [R, N], partials [R / 16, N]): dz = (dy_e @ w_e) * gelu_tanh'(z) on group e's rows (w [E, K, N] read in place),
+// other rows zero; the partial rows of each group's ceil(count / 16) row blocks (reduce with grouped_column_sum).
+std::tuple<Tensor, Tensor> grouped_gemm_nn_gelu_backward(const Tensor& dy, const Tensor& w, const Tensor& z,
+                                                         const Tensor& counts) {
+  TORCH_CHECK(grouped_gemm_nn_ok(dy, w, counts) && bf16_2d(z) && z.device() == dy.device() && z.size(0) == dy.size(0) &&
+                  z.size(1) == w.size(2),
+              "mpi4torch_b200: grouped_gemm_nn_gelu_backward needs contiguous bf16 dy [R, K], w [E, K, N] and z [R, N]",
+              kGroupedRules);
+  c10::cuda::CUDAGuard guard(dy.device());
+  const int64_t R = dy.size(0), N = w.size(2);
+  Tensor dz = at::empty({R, N}, dy.options());
+  Tensor part = at::empty({colsum_rows(R), N}, dy.options().dtype(at::kFloat));
+  std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
+  launch_gemm_nn_gelu_bwd_colsum_grouped(dy.data_ptr(), w.data_ptr(), z.data_ptr(), dz.data_ptr(), part.data_ptr<float>(),
+                                         counts.data_ptr<int>(), w.size(0), R, N, dy.size(1), sm_count(), stream_of(dy));
+  return {dz, part};
+}
+
+// c [R, N] = a_e @ b_e on group e's rows (b [E, K, N] read in place), other rows zero.  One launch.
+Tensor grouped_gemm_nn(const Tensor& a, const Tensor& b, const Tensor& counts) {
+  TORCH_CHECK(grouped_gemm_nn_ok(a, b, counts),
+              "mpi4torch_b200: grouped_gemm_nn needs contiguous bf16 a [R, K] and b [E, K, N]", kGroupedRules);
+  c10::cuda::CUDAGuard guard(a.device());
+  Tensor c = at::empty({a.size(0), b.size(2)}, a.options());
+  std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
+  launch_gemm_nn_grouped(a.data_ptr(), b.data_ptr(), c.data_ptr(), counts.data_ptr<int>(), b.size(0), a.size(0), b.size(2),
+                         a.size(1), sm_count(), stream_of(a));
+  return c;
+}
+
+// G [E, N, K]: G_e = grad_scale * dy_e^T @ x_e over group e's rows; zero for an empty group.  One launch.
+Tensor grouped_wgrad_bf16(const Tensor& dy, const Tensor& x, const Tensor& counts, const c10::optional<Tensor>& grad_scale) {
+  TORCH_CHECK(grouped_wgrad_bf16_ok(dy, x, counts),
+              "mpi4torch_b200: grouped_wgrad_bf16 needs contiguous bf16 dy [R, N] and x [R, K]", kGroupedRules);
+  c10::cuda::CUDAGuard guard(x.device());
+  Tensor gw = at::empty({counts.size(0), dy.size(1), x.size(1)}, x.options());
+  std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
+  launch_wgrad_bf16_grouped(dy.data_ptr(), x.data_ptr(), gw.data_ptr(), counts.data_ptr<int>(), counts.size(0), dy.size(0),
+                            dy.size(1), x.size(1), sm_count(), stream_of(x), grad_scale_ptr(grad_scale, x));
+  return gw;
+}
+
+// out [E, N] fp32: per group, the sum of its column-sum partial rows (partials [R / 16, N] fp32, R = rows of the
+// grouped tensor) or, for a bf16 [R, N] input, of its valid rows.  Fixed order, no atomics.  One launch.
+Tensor grouped_column_sum(const Tensor& in, const Tensor& counts) {
+  const bool bf16_rows = in.scalar_type() == at::kBFloat16;
+  const int64_t rows = in.dim() == 2 ? (bf16_rows ? 1 : 16) * in.size(0) : 0;  // R
+  TORCH_CHECK(in.is_cuda() && in.dim() == 2 && in.is_contiguous() && (bf16_rows || in.scalar_type() == at::kFloat) &&
+                  counts_ok(counts, in) && counts.size(0) <= 1024 && rows > 0 && rows % 128 == 0 && in.size(1) > 0,
+              "mpi4torch_b200: grouped_column_sum needs bf16 rows [R, N] or fp32 partials [R / 16, N] (contiguous, "
+              "R % 128 == 0) and contiguous int32 counts [E <= 1024] on the same CUDA device");
+  c10::cuda::CUDAGuard guard(in.device());
+  Tensor out = at::empty({counts.size(0), in.size(1)}, in.options().dtype(at::kFloat));
+  launch_column_sum_grouped(in.data_ptr(), bf16_rows, counts.data_ptr<int>(), counts.size(0), rows, in.size(1),
+                            out.data_ptr<float>(), stream_of(in));
+  return out;
+}
+
 // ---- FP8 linear layer (gemm_fp8.cu) ------------------------------------------------------------------------------
 bool fp8_e5m2(c10::string_view fmt) {
   TORCH_CHECK(fmt == "e4m3" || fmt == "e5m2", "mpi4torch_b200: the fp8 format must be 'e4m3' or 'e5m2'");
@@ -701,6 +833,17 @@ TORCH_LIBRARY_FRAGMENT(mpi4torch_b200, m) {
   m.def("batched_gemm_nn(Tensor a, Tensor b) -> Tensor", &batched_gemm_nn);
   m.def("batched_wgrad_bf16(Tensor dy, Tensor x, Tensor? grad_scale=None) -> Tensor", &batched_wgrad_bf16);
   m.def("batched_column_sum(Tensor partials, Tensor? grad_scale=None) -> Tensor", &batched_column_sum);
+  m.def("grouped_gemm_tn_supported(Tensor x, Tensor w, Tensor counts, Tensor? bias=None) -> bool", &grouped_gemm_tn_ok);
+  m.def("grouped_gemm_nn_supported(Tensor a, Tensor b, Tensor counts) -> bool", &grouped_gemm_nn_ok);
+  m.def("grouped_wgrad_bf16_supported(Tensor dy, Tensor x, Tensor counts) -> bool", &grouped_wgrad_bf16_ok);
+  m.def("grouped_linear_bias_gelu_forward(Tensor x, Tensor w, Tensor b, Tensor counts) -> (Tensor, Tensor)",
+        &grouped_linear_bias_gelu_forward);
+  m.def("grouped_linear_bias_forward(Tensor x, Tensor w, Tensor b, Tensor counts) -> Tensor", &grouped_linear_bias_forward);
+  m.def("grouped_gemm_nn_gelu_backward(Tensor dy, Tensor w, Tensor z, Tensor counts) -> (Tensor, Tensor)",
+        &grouped_gemm_nn_gelu_backward);
+  m.def("grouped_gemm_nn(Tensor a, Tensor b, Tensor counts) -> Tensor", &grouped_gemm_nn);
+  m.def("grouped_wgrad_bf16(Tensor dy, Tensor x, Tensor counts, Tensor? grad_scale=None) -> Tensor", &grouped_wgrad_bf16);
+  m.def("grouped_column_sum(Tensor partials, Tensor counts) -> Tensor", &grouped_column_sum);
   m.def("linear_bias_gelu_forward(Tensor x, Tensor w, Tensor b) -> (Tensor, Tensor)", &linear_bias_gelu_forward);
   m.def("linear_bias_mse_forward_local(Tensor x, Tensor w, Tensor b, Tensor target, float loss_scale, float grad_scale) "
         "-> (Tensor, Tensor, Tensor)",

@@ -47,11 +47,17 @@ struct GemmArgs {
   float* loss_acc;
   float loss_scale, grad_scale;
   // fused mode ----------------------------------------------------------------
-  const uint32_t* panel_flags;  // [N / kPanel] counters in local HBM (written through multicast)
+  union {
+    const uint32_t* panel_flags;  // [N / kPanel] counters in local HBM (written through multicast)
+    const int* group_counts;      // GROUPED (never fused): [groups] rows of each group, int32 on the device
+  };
   uint32_t panel_target;        // a panel is ready when its counter >= target (wrap-safe)
-  // batched kernels: rows of one expert (a multiple of BM).  Placed in the tail padding, so the other
-  // kernels' parameter layout is unchanged.
-  int expert_rows;
+  // batched kernels: rows of one expert (a multiple of BM); grouped kernels: the number of groups.  Placed in the
+  // tail padding, so the other kernels' parameter layout is unchanged.
+  union {
+    int expert_rows;
+    int groups;
+  };
 };
 
 // Epilogues of the two-layer MLP (unused by kStore / kMse):
@@ -266,12 +272,106 @@ __device__ __forceinline__ void xent_epilogue(float (&acc)[BN / 2], const GemmAr
   }
 }
 
+// Grouped tiles: this warpgroup's rows at or past `valid` (an absolute row) of the tile become zero in C, and in
+// h_out for kBiasGelu.  C is [g.M, g.N] contiguous with g.M a multiple of BM, so every row of the tile exists.
+template <int EPI, int BN>
+__device__ __forceinline__ void zero_rows_epilogue(const GemmArgs& g, const MlpEpiArgs& e, int m_blk, int n_blk, int wgi,
+                                                   int valid) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = m_blk * BM + wgi * 64 + frag_row(h);
+    if (row < valid) continue;
+    const int64_t off = static_cast<int64_t>(row) * g.ldc;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int col = n_blk * BN + frag_col(j);
+      if (col >= g.N) break;
+      *reinterpret_cast<uint32_t*>(static_cast<uint16_t*>(g.C) + off + col) = 0u;
+      if (EPI == kBiasGelu) *reinterpret_cast<uint32_t*>(static_cast<uint16_t*>(e.h_out) + off + col) = 0u;
+    }
+  }
+}
+
+// Tile t of the grouped kernel: the used * n_tiles tiles of the groups come first, M fastest, then the zero tiles of the
+// m-blocks behind the last group, so the persistent CTAs share the real tiles evenly.
+__device__ __forceinline__ void grouped_tile(int t, int m_tiles, int used, int n_tiles, int& m_blk, int& n_blk) {
+  const int live = used * n_tiles;
+  if (t < live) {
+    n_blk = t / used;
+    m_blk = t - n_blk * used;
+  } else {
+    const int z = t - live, rest = m_tiles - used;
+    n_blk = z / rest;
+    m_blk = used + (z - n_blk * rest);
+  }
+}
+
+// Producer and consumer roles of the grouped kernel (see gemm_bf16_wgmma_kernel).  A tile of group ge reads B at row
+// offset ge * (N, or K if B_MN), the bias at ge * N, and stores its rows below the group's end.
+template <int EPI, bool B_MN, int BN>
+__device__ __forceinline__ void grouped_roles(uint8_t* smem, Pipe* pipe, const CUtensorMap* tmap_a,
+                                              const CUtensorMap* tmap_b, const GemmArgs& g, const MlpEpiArgs& e,
+                                              int first_tile, int tile_stride, int m_tiles, int num_tiles, int k_blocks) {
+  const GroupTable* grp = group_table_of(pipe);
+  const int n_tiles = num_tiles / m_tiles;
+  const int warp = threadIdx.x >> 5;
+  const int used = grp->pfx[g.groups];  // m-blocks holding groups; the rest are zero tiles
+  if (warp < 4) {
+    if constexpr (epi_reallocs(EPI)) tc::setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int t = first_tile; t < used * n_tiles; t += tile_stride) {
+        int m_blk, n_blk;
+        grouped_tile(t, m_tiles, used, n_tiles, m_blk, n_blk);
+        const int b_row0 = group_of(grp, g.groups, m_blk) * (B_MN ? g.K : g.N);
+        for (int kb = 0; kb < k_blocks; ++kb)
+          load_stage<false, B_MN, BN>(smem, pipe, stage, phase, tmap_a, tmap_b, m_blk * BM, n_blk * BN, kb * BK, b_row0);
+      }
+    }
+  } else {
+    if constexpr (epi_reallocs(EPI)) tc::setmaxnreg_inc<232>();
+    const int wgi = warp / 4 - 1;
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[BN / 2];
+    for (int t = first_tile; t < num_tiles; t += tile_stride) {
+      int m_blk, n_blk;
+      grouped_tile(t, m_tiles, used, n_tiles, m_blk, n_blk);
+      int valid = m_blk * BM;  // rows below this one are stored from acc, the tile's others as zero
+      if (m_blk < used) {
+        const int ge = group_of(grp, g.groups, m_blk);
+        valid = grp->end[ge];
+        mma_tile<false, B_MN, BN>(acc, smem, pipe, stage, phase, k_blocks, wgi);
+        GemmArgs gg = g;
+        gg.M = valid;
+        if constexpr (EPI == kStore) {
+          store_epilogue<EPI, BN>(acc, gg, m_blk, n_blk, wgi);
+        } else {
+          float unused = 0.f;
+          MlpEpiArgs ex = e;
+          if (e.bias != nullptr) ex.bias = e.bias + static_cast<int64_t>(ge) * g.N;
+          mlp_epilogue<EPI, BN>(acc, gg, ex, m_blk, n_blk, wgi, unused);
+        }
+      }
+      zero_rows_epilogue<EPI, BN>(g, e, m_blk, n_blk, wgi, valid);
+    }
+  }
+}
+
 // BATCHED: E experts stacked along M (g.M = E * g.expert_rows); the tile's expert is m0 / expert_rows.  Only B and
 // the bias depend on it: B is one map over the stacked weights, read at row offset expert * (N, or K if B_MN).
-template <bool FUSED, int EPI, bool B_MN, bool BATCHED = false>
+// GROUPED: g.groups groups of g.group_counts[e] rows in the grouped layout of the g.M rows (GroupTable, built once per
+// CTA in shared memory).  The tile space is every m-block of g.M (grouped_tile): a tile's group comes from the table,
+// its rows at or past the group's count are stored as zero, and m-blocks behind the last group are zero tiles that
+// load nothing and come after all the others.  Epilogues kStore, kBiasGelu, kGeluBwdColsum and kBias.
+template <bool FUSED, int EPI, bool B_MN, bool BATCHED = false, bool GROUPED = false>
 __global__ void __launch_bounds__(kGemmThreads + (FUSED ? kCommWarps * 32 : 0), 1)
 gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                        const GemmArgs g, const CommArgs cm, const MlpEpiArgs e) {
+  static_assert(!GROUPED || (!FUSED && !BATCHED && (EPI == kStore || EPI == kBiasGelu || EPI == kGeluBwdColsum ||
+                                                    EPI == kBias)),
+                "grouped GEMM epilogues");
   constexpr int BN = tile_n<FUSED>();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = aligned_smem(smem_raw);
@@ -291,7 +391,16 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     tc::prefetch_tmap(&tmap_b);
     init_pipe<BN>(pipe);
   }
+  if constexpr (GROUPED) {
+    if (threadIdx.x == 32) build_group_table(group_table_of(pipe), g.group_counts, g.groups, g.M);
+  }
   __syncthreads();
+  if constexpr (GROUPED) {
+    grouped_roles<EPI, B_MN, BN>(smem, pipe, &tmap_a, &tmap_b, g, e, first_tile, tile_stride, m_tiles, num_tiles,
+                                 k_blocks);
+    __syncthreads();
+    return;
+  }
 
   if (warp < 4) {
     // =========================== TMA producer ===========================
@@ -359,14 +468,15 @@ CUtensorMap make_tmap(const void* base, int64_t rows, int64_t cols, int64_t ld, 
 
 // ctas: the SM count, of which the persistent grid uses no more than g has tiles; the fused kernel's grid
 // (fused_gemm_grid), which it uses whole.
-template <bool FUSED, int EPI, bool B_MN, bool BATCHED = false>
+template <bool FUSED, int EPI, bool B_MN, bool BATCHED = false, bool GROUPED = false>
 void launch(int ctas, const CUtensorMap& ta, const CUtensorMap& tb, const GemmArgs& g, cudaStream_t stream,
             const char* what, const MlpEpiArgs& e = MlpEpiArgs{}, const CommArgs& cm = CommArgs{}) {
   constexpr int BN = tile_n<FUSED>();
   const int64_t M = g.M, N = g.N;
   const int grid = FUSED ? ctas : persistent_grid(((M + BM - 1) / BM) * ((N + BN - 1) / BN), ctas);
-  launch_kernel<gemm_bf16_wgmma_kernel<FUSED, EPI, B_MN, BATCHED>>(grid, kGemmThreads + (FUSED ? kCommWarps * 32 : 0),
-                                                                     Tile<BN>::kSmemBytes, stream, what, ta, tb, g, cm, e);
+  launch_kernel<gemm_bf16_wgmma_kernel<FUSED, EPI, B_MN, BATCHED, GROUPED>>(
+      grid, kGemmThreads + (FUSED ? kCommWarps * 32 : 0), Tile<BN>::kSmemBytes + (GROUPED ? kGroupTableBytes : 0), stream,
+      what, ta, tb, g, cm, e);
 }
 
 void set_mse(GemmArgs& g, const MseEpilogue* mse) {
@@ -766,6 +876,129 @@ void launch_column_sum_batched(const float* partial, int64_t E, int64_t rows, in
   const dim3 grid(static_cast<unsigned>((N + 31) / 32), static_cast<unsigned>(E));
   launch_kernel<column_sum_kernel<true>>(grid, 256, 0, stream, "column_sum_batched", partial, static_cast<int>(rows),
                                          static_cast<int>(N), out, gscale);
+}
+
+// ---- grouped experts ---------------------------------------------------------------------------------------------
+// A [R, K] in the grouped layout of `counts` (GroupTable), B [E, N, K] (TN) or [E, K, N] (NN), C [R, N], bias [E, N].
+// The tile space is all R / 128 m-blocks, so C is fully written: rows past a group's count and behind the last group
+// are zero.
+namespace {
+
+GemmArgs grouped_args(void* C, const int* counts, int64_t E, int64_t R, int64_t N, int64_t K) {
+  GemmArgs g = plain_args(C, R, N, K, N);
+  g.group_counts = counts;
+  g.groups = static_cast<int>(E);
+  return g;
+}
+
+// Expert e sums rows [first_e, first_e + n_e) of in [.., N] (fp32, or bf16 read as fp32) into out[e] in column_sum's
+// order, with first_e = start_e / row_div and n_e = ceil((end_e - start_e) / row_div) from the grouped layout of
+// `counts` over R rows.  row_div 16 reduces the GELU-backward epilogue's column-sum partials, row_div 1 the rows
+// themselves.  No atomics: the same bits on every call.
+template <typename T>
+__global__ void __launch_bounds__(256) grouped_column_sum_kernel(const T* __restrict__ in, int N, const int* counts,
+                                                                 int R, int row_div, float* __restrict__ out) {
+  __shared__ float part[8][33];
+  __shared__ int span[2];
+  if (threadIdx.x == 0) {
+    int p = 0, start = 0, end = 0;
+    for (int e = 0; e <= static_cast<int>(blockIdx.y); ++e) {  // build_group_table's rule, up to this group
+      const int c = min(max(counts[e], 0), R);
+      start = p * BM;
+      p = min(p + (c + BM - 1) / BM, R / BM);
+      end = min(start + c, R);
+    }
+    span[0] = start / row_div;
+    span[1] = (end - start + row_div - 1) / row_div;
+  }
+  __syncthreads();
+  const int first = span[0], rows = span[1];
+  out += static_cast<int64_t>(blockIdx.y) * N;
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  const int n = blockIdx.x * 32 + tx;
+  float s = 0.f;
+  if (n < N)
+    for (int i = ty; i < rows; i += 8) {
+      const T v = in[static_cast<int64_t>(first + i) * N + n];
+      if constexpr (sizeof(T) == 2) s += bf16_bits_to_float(v);
+      else s += v;
+    }
+  part[ty][tx] = s;
+  __syncthreads();
+  if (ty == 0 && n < N) {
+    float t = part[0][tx];
+#pragma unroll
+    for (int k = 1; k < 8; ++k) t += part[k][tx];
+    out[n] = t;
+  }
+}
+
+}  // namespace
+
+bool grouped_gemm_supported(int64_t E, int64_t R, int64_t N, int64_t K, const void* A, const void* B, const void* C,
+                            const void* counts) {
+  return E > 0 && E <= kMaxGroups && R > 0 && N > 0 && K > 0 && R % BM == 0 && N % 128 == 0 && K % 128 == 0 &&
+         aligned16(A) && aligned16(B) && aligned16(C) && (reinterpret_cast<uintptr_t>(counts) & 3u) == 0 &&
+         R < (1ll << 31) && R / BM * ((N + tile_n<false>() - 1) / tile_n<false>()) < (1ll << 31) && E * N < (1ll << 31) &&
+         E * K < (1ll << 31);
+}
+
+void launch_gemm_bias_gelu_grouped(const void* A, const void* B, const float* bias, void* z, void* h, const int* counts,
+                                   int64_t E, int64_t R, int64_t N, int64_t K, int sm_count, cudaStream_t stream) {
+  M4T_CHECK(grouped_gemm_supported(E, R, N, K, A, B, z, counts) && aligned16(h) && epilogue_bias_ok(bias),
+            "unsupported shape/alignment for the grouped bias+GELU GEMM");
+  MlpEpiArgs e{};
+  e.bias = bias;
+  e.h_out = h;
+  launch<false, kBiasGelu, false, false, true>(sm_count, make_tmap(A, R, K, K, BM), make_tmap(B, E * N, K, K, tile_n<false>()),
+                                               grouped_args(z, counts, E, R, N, K), stream, "gemm_bias_gelu_grouped", e);
+}
+
+void launch_gemm_bias_grouped(const void* A, const void* B, const float* bias, void* y, const int* counts, int64_t E,
+                              int64_t R, int64_t N, int64_t K, int sm_count, cudaStream_t stream) {
+  M4T_CHECK(grouped_gemm_supported(E, R, N, K, A, B, y, counts) && epilogue_bias_ok(bias),
+            "unsupported shape/alignment for the grouped bias GEMM");
+  MlpEpiArgs e{};
+  e.bias = bias;
+  launch<false, kBias, false, false, true>(sm_count, make_tmap(A, R, K, K, BM), make_tmap(B, E * N, K, K, tile_n<false>()),
+                                           grouped_args(y, counts, E, R, N, K), stream, "gemm_bias_grouped", e);
+}
+
+void launch_gemm_nn_gelu_bwd_colsum_grouped(const void* A, const void* B, const void* z, void* dz, float* colsum,
+                                            const int* counts, int64_t E, int64_t R, int64_t N, int64_t K, int sm_count,
+                                            cudaStream_t stream) {
+  M4T_CHECK(grouped_gemm_supported(E, R, N, K, A, B, dz, counts) && epilogue_bf16_pairs_ok(z, N),
+            "unsupported shape/alignment for the grouped GELU-backward GEMM");
+  GemmArgs g = grouped_args(dz, counts, E, R, N, K);
+  g.T = z;
+  g.ldt = static_cast<int>(N);
+  MlpEpiArgs e{};
+  e.colsum = colsum;
+  launch<false, kGeluBwdColsum, true, false, true>(sm_count, make_tmap(A, R, K, K, BM),
+                                                   make_tmap_bf16_sw128(B, E * K, N, N, 64, BK), g, stream,
+                                                   "gemm_nn_gelu_bwd_colsum_grouped", e);
+}
+
+void launch_gemm_nn_grouped(const void* A, const void* B, void* C, const int* counts, int64_t E, int64_t R, int64_t N,
+                            int64_t K, int sm_count, cudaStream_t stream) {
+  M4T_CHECK(grouped_gemm_supported(E, R, N, K, A, B, C, counts), "unsupported shape/alignment for the grouped NN GEMM");
+  launch<false, kStore, true, false, true>(sm_count, make_tmap(A, R, K, K, BM), make_tmap_bf16_sw128(B, E * K, N, N, 64, BK),
+                                           grouped_args(C, counts, E, R, N, K), stream, "gemm_nn_grouped");
+}
+
+void launch_column_sum_grouped(const void* in, bool bf16_rows, const int* counts, int64_t E, int64_t R, int64_t N,
+                               float* out, cudaStream_t stream) {
+  M4T_CHECK(E > 0 && E <= kMaxGroups && R > 0 && R % BM == 0 && N > 0 && R * N < (1ll << 31),
+            "column_sum_grouped: empty or oversized input");
+  const dim3 grid(static_cast<unsigned>((N + 31) / 32), static_cast<unsigned>(E));
+  if (bf16_rows)
+    launch_kernel<grouped_column_sum_kernel<uint16_t>>(grid, 256, 0, stream, "row_sum_grouped",
+                                                       static_cast<const uint16_t*>(in), static_cast<int>(N), counts,
+                                                       static_cast<int>(R), 1, out);
+  else
+    launch_kernel<grouped_column_sum_kernel<float>>(grid, 256, 0, stream, "column_sum_grouped",
+                                                    static_cast<const float*>(in), static_cast<int>(N), counts,
+                                                    static_cast<int>(R), 16, out);
 }
 
 }  // namespace m4t

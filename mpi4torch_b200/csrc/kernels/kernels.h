@@ -226,6 +226,34 @@ bool wgrad_bf16_batched_supported(int64_t E, int64_t Mb, int64_t N, int64_t K, c
 void launch_wgrad_bf16_batched(const void* dy, const void* x, void* g, int64_t E, int64_t Mb, int64_t N, int64_t K,
                                int sm_count, cudaStream_t stream, const float* gscale = nullptr);
 
+// ---- grouped experts (gemm_wgmma.cu, wgrad_wgmma.cu; DESIGN §4.4) -------------------------------------------------
+// E experts with row counts `counts` [E] (int32, read on the device only) share one [R, .] operand in the grouped
+// layout: expert e's rows start at row 128 * sum_{j<e} ceil(counts[j] / 128).  Counts are clamped to [0, R]; rows of
+// a group that would lie past R do not exist.  Weights are stacked as for the batched kernels: B [E, N, K] (TN) or
+// [E, K, N] (NN), bias [E, N].  Outputs [R, N] are written whole: rows past a group's count and behind the last group
+// are zero.  R % 128 == N % 128 == K % 128 == 0, 1 <= E <= 1024, 16-byte-aligned operands.
+bool grouped_gemm_supported(int64_t E, int64_t R, int64_t N, int64_t K, const void* A, const void* B, const void* C,
+                            const void* counts);
+void launch_gemm_bias_gelu_grouped(const void* A, const void* B, const float* bias, void* z, void* h, const int* counts,
+                                   int64_t E, int64_t R, int64_t N, int64_t K, int sm_count, cudaStream_t stream);
+void launch_gemm_bias_grouped(const void* A, const void* B, const float* bias, void* y, const int* counts, int64_t E,
+                              int64_t R, int64_t N, int64_t K, int sm_count, cudaStream_t stream);
+// colsum: [R / 16, N] partials; the rows of group e's ceil(count / 16) partial rows are written, the others are not.
+void launch_gemm_nn_gelu_bwd_colsum_grouped(const void* A, const void* B, const void* z, void* dz, float* colsum,
+                                            const int* counts, int64_t E, int64_t R, int64_t N, int64_t K, int sm_count,
+                                            cudaStream_t stream);
+void launch_gemm_nn_grouped(const void* A, const void* B, void* C, const int* counts, int64_t E, int64_t R, int64_t N,
+                            int64_t K, int sm_count, cudaStream_t stream);
+// out [E, N] fp32: per group, the sum of its column-sum partial rows ([R / 16, N] fp32), or of its valid rows
+// (bf16_rows: [R, N] bf16), in column_sum's fixed order.
+void launch_column_sum_grouped(const void* in, bool bf16_rows, const int* counts, int64_t E, int64_t R, int64_t N,
+                               float* out, cudaStream_t stream);
+// G_e [N, K] = gscale * dY_e^T X_e over group e's rows of dY [R, N] and X [R, K]; G [E, N, K], zero for an empty group.
+bool wgrad_bf16_grouped_supported(int64_t E, int64_t R, int64_t N, int64_t K, const void* dy, const void* x,
+                                  const void* g, const void* counts);
+void launch_wgrad_bf16_grouped(const void* dy, const void* x, void* g, const int* counts, int64_t E, int64_t R,
+                               int64_t N, int64_t K, int sm_count, cudaStream_t stream, const float* gscale = nullptr);
+
 // ---- FP8 training of the linear layer (gemm_fp8.cu, DESIGN §4.4) ---------------------------------------------
 // Per-tensor power-of-two scaling: amax of a bf16 [rows, cols] matrix (leading dimension ld) -> *amax_bits (the bit
 // pattern of the fp32 amax; zeroed by the caller, atomicMax), then q = fp8(v * s) row-major [rows, cols] and/or

@@ -90,17 +90,42 @@ __device__ __forceinline__ void load_stage(uint8_t* smem, Pipe* p, int& stage, u
   advance<BN>(stage, phase);
 }
 
+// Rows [rows, BK) of every 64-row MN-major box of a stage become zero, so the k-block contracts over its first
+// `rows` rows only.  Both operands: a zero in one alone would still give 0 * NaN = NaN.  The two consumer warpgroups
+// (256 threads) share the work, order their generic-proxy stores before the wgmma's async-proxy reads, and meet on
+// named barrier 2 (the fused kernels' communication warps use barrier 1), so neither reads a row the other has not
+// yet cleared.  A 128-byte swizzled row holds exactly one k-row of a box, so the swizzle does not matter here.
+template <int BN>
+__device__ __forceinline__ void zero_stage_rows(uint8_t* stage_base, int rows) {
+  constexpr int kBoxes = Tile<BN>::kStageBytes / kBoxBytesMN;
+  // consumer thread t clears 16-byte piece t % 8 of rows rows + t / 8, rows + t / 8 + 32 .. of every box
+  const int t = static_cast<int>(threadIdx.x) - 128;
+  for (int r = rows + (t >> 3); r < BK; r += kConsumerWarps * 32 / 8) {
+    uint8_t* p = stage_base + r * 128 + (t & 7) * 16;
+#pragma unroll
+    for (int box = 0; box < kBoxes; ++box) *reinterpret_cast<uint4*>(p + box * kBoxBytesMN) = make_uint4(0, 0, 0, 0);
+  }
+  tc::fence_proxy_async();
+  asm volatile("bar.sync 2, %0;" ::"n"(kConsumerWarps * 32) : "memory");
+}
+
 // Consumer warpgroup `wgi` (0/1): acc = its 64 rows of the tile, summed over k_blocks stages.
 // The stage of k-block kb is handed back to the producer once the wgmma of kb + 1 has been
 // issued and those of kb have retired (wait_group 1), so one k-block of MMAs is always queued.
-template <bool A_MN, bool B_MN, int BN>
+// TAIL_ROWS (both operands MN-major): the last k-block contracts over its first tail_rows rows only
+// (zero_stage_rows), the grouped wgrad's last k-block of a group.
+template <bool A_MN, bool B_MN, int BN, bool TAIL_ROWS = false>
 __device__ __forceinline__ void mma_tile(float (&acc)[BN / 2], uint8_t* smem, Pipe* p, int& stage, uint32_t& phase,
-                                         int k_blocks, int wgi) {
+                                         int k_blocks, int wgi, int tail_rows = BK) {
+  static_assert(!TAIL_ROWS || (A_MN && B_MN), "row masking needs MN-major boxes");
   const int lane = threadIdx.x & 31;
   int prev = -1;
   tc::fence_regs(acc);
   for (int kb = 0; kb < k_blocks; ++kb) {
     tc::mbar_wait(&p->full[stage], phase);
+    if constexpr (TAIL_ROWS) {
+      if (kb == k_blocks - 1 && tail_rows < BK) zero_stage_rows<BN>(smem + stage * Tile<BN>::kStageBytes, tail_rows);
+    }
     const uint32_t sa = tc::smem_u32(smem + stage * Tile<BN>::kStageBytes);
     const uint32_t sb = sa + kABytes;
     // this warpgroup's 64 rows of A: one MN-major box, or 64 K-major rows of 128 bytes
@@ -159,6 +184,46 @@ __device__ __forceinline__ void mma_tile_fp8(float (&acc)[64], uint8_t* smem, Pi
     for (int i = 0; i < 64; ++i) acc[i] += blk[i];
     advance<128>(stage, phase);
   }
+}
+
+// ---- grouped layout (DESIGN §4.4) --------------------------------------------------------------------------------
+// E groups with device-resident row counts c_e share one [rows, .] operand: group e starts at row BM * pfx[e] with
+// pfx[e] = sum_{j<e} ceil(c_j / BM), so no BM-row tile spans two groups.  Counts are clamped to [0, rows] and pfx to
+// rows / BM: a group (or its part) past the last row has no rows, and nothing outside the operands is touched.
+constexpr int kMaxGroups = 1024;
+struct GroupTable {
+  int pfx[kMaxGroups + 1];  // first m-block of each group; pfx[E] = m-blocks in use
+  int end[kMaxGroups];      // one past the group's last valid row
+};
+// Bytes a grouped kernel adds to its dynamic shared memory (the table sits behind the ring's barriers).
+constexpr int kGroupTableBytes = static_cast<int>(sizeof(GroupTable));
+__device__ __forceinline__ GroupTable* group_table_of(Pipe* pipe) {
+  return reinterpret_cast<GroupTable*>(reinterpret_cast<uint8_t*>(pipe) + 256);
+}
+
+// One thread builds the table; the kernel's first __syncthreads publishes it.
+__device__ __forceinline__ void build_group_table(GroupTable* t, const int* counts, int E, int rows) {
+  const int cap = rows / BM;
+  int p = 0;
+  t->pfx[0] = 0;
+  for (int e = 0; e < E; ++e) {
+    const int c = min(max(counts[e], 0), rows);
+    const int start = p * BM;
+    p = min(p + (c + BM - 1) / BM, cap);
+    t->pfx[e + 1] = p;
+    t->end[e] = min(start + c, rows);
+  }
+}
+
+// The group whose m-blocks hold m_blk (m_blk < pfx[E]): the last e with pfx[e] <= m_blk, which skips empty groups.
+__device__ __forceinline__ int group_of(const GroupTable* t, int E, int m_blk) {
+  int lo = 0, hi = E - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (t->pfx[mid] <= m_blk) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
 }
 
 // Accumulator fragment of wgmma m64nN (fp32): thread (warp w of the warpgroup, lane l) holds, for

@@ -49,11 +49,15 @@ struct WgradArgs {
                         // the heaps of WgradComm)
   int Mb, N, K;
   int ldo;              // leading dimension of out (elements)
-  int ksplit;
+  union {
+    int ksplit;
+    const int* group_counts;  // GROUPED (ksplit 1): [experts] rows of each group, int32 on the device.  The slot of
+                              // ksplit and its padding, so the parameter layout is unchanged.
+  };
   const float* gscale;  // optional device scalar multiplied into every output element (the upstream
                         // gradient of the loss: autograd hands it over as a tensor, never through the host)
   float axpy;           // plain mode with axpy != 0: out <- out + axpy * gscale * G  (single-rank SGD epilogue)
-  int experts;          // BATCHED: E (in the tail padding: the other kernels' parameter layout is unchanged)
+  int experts;          // BATCHED, GROUPED: E (in the tail padding: the other kernels' parameter layout is unchanged)
 };
 
 struct WgradComm {
@@ -349,15 +353,81 @@ __device__ __forceinline__ void acc32_epilogue(const float (&acc)[BN / 2], char*
   }
 }
 
+// The grouped wgrad (wgrad_bf16_wgmma_kernel with GROUPED): tile t of E * n_tiles * k_tiles is (expert, n, k) as in the
+// batched kernel, contracted over the expert's rows [128 pfx[e], end[e]) of the grouped layout.
+template <int BN>
+__device__ __forceinline__ void grouped_wgrad_roles(uint8_t* smem, Pipe* pipe, const CUtensorMap* tmap_a,
+                                                    const CUtensorMap* tmap_b, const WgradArgs& g, int n_tiles,
+                                                    int k_tiles) {
+  GroupTable* grp = group_table_of(pipe);
+  const int warp = threadIdx.x >> 5;
+  if (threadIdx.x == 0) {
+    tc::prefetch_tmap(tmap_a);
+    tc::prefetch_tmap(tmap_b);
+    init_pipe<BN>(pipe);
+  }
+  if (threadIdx.x == 32) build_group_table(grp, g.group_counts, g.experts, g.Mb);
+  __syncthreads();
+  const int num_tiles = n_tiles * k_tiles * g.experts;
+  if (warp < 4) {
+    if (threadIdx.x == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+        const int n_blk = t / k_tiles;
+        const int k_blk = t - n_blk * k_tiles;
+        const int expert = n_blk / n_tiles;
+        const int row0 = grp->pfx[expert] * BM;
+        const int kbs = (max(grp->end[expert] - row0, 0) + BK - 1) / BK;
+        for (int kb = 0; kb < kbs; ++kb)
+          load_stage<true, true, BN>(smem, pipe, stage, phase, tmap_a, tmap_b, (n_blk - expert * n_tiles) * BM,
+                                     k_blk * BN, row0 + kb * BK);
+      }
+    }
+  } else {
+    const int wgi = warp / 4 - 1;
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[BN / 2];
+    const float gs = g.gscale ? __ldg(g.gscale) : 1.0f;
+    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+      const int n_blk = t / k_tiles;
+      const int k_blk = t - n_blk * k_tiles;
+      const int expert = n_blk / n_tiles;
+      const int rows = max(grp->end[expert] - grp->pfx[expert] * BM, 0);
+      const int kbs = (rows + BK - 1) / BK;
+      if (kbs > 0) {
+        mma_tile<true, true, BN, true>(acc, smem, pipe, stage, phase, kbs, wgi, rows - (kbs - 1) * BK);
+        bf16_epilogue<BN>(acc, static_cast<char*>(g.out), g.ldo, g.K, gs, false, n_blk, k_blk, wgi);
+        continue;
+      }
+      // an expert without rows: a zero gradient (zeroing acc instead makes ptxas spill it)
+      const int cols = min(BN, g.K - k_blk * BN);
+#pragma unroll 1
+      for (int hr = 0; hr < 2; ++hr) {
+        uint16_t* orow = static_cast<uint16_t*>(g.out) + static_cast<int64_t>(n_blk * BM + wgi * 64 + frag_row(hr)) * g.ldo +
+                         k_blk * BN;
+#pragma unroll 1
+        for (int j = 0; j < cols / 8; ++j) *reinterpret_cast<uint32_t*>(orow + frag_col(j)) = 0u;
+      }
+    }
+  }
+  __syncthreads();
+}
+
 // ACC32 (plain mode only): out is an fp32 [N, K] buffer and the epilogue is out <- fmaf(gscale, G, out), the
 // gradient accumulation of micro-batches.  A compile-time mode, so the other instantiations are unchanged.
 // BATCHED (plain mode only): E = g.experts problems G_e = dY_e^T X_e of the same shape, with dY [E Mb, N], X [E Mb, K]
 // and out [E N, K] stacked.  Tile rows of the stacked output run over E * N / 128 blocks: block n_blk belongs to
 // expert n_blk / (N / 128), whose contraction rows start at row expert * Mb of both operands.
-template <bool FUSED, bool ACC32 = false, bool BATCHED = false>
+// GROUPED (plain mode only): the same tiles and output, with dY [Mb, N] and X [Mb, K] in the grouped layout of
+// g.group_counts over Mb rows (GroupTable).  Expert e contracts over the ceil(rows_e / 64) k-blocks from its first
+// row; the last one's rows past the group are zeroed in both operands, and an expert without rows stores zeros.
+template <bool FUSED, bool ACC32 = false, bool BATCHED = false, bool GROUPED = false>
 __global__ void __launch_bounds__(kGemmThreads + (FUSED ? kCommWarps * 32 : 0), 1)
 wgrad_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                         const WgradArgs g, const WgradComm wc) {
+  static_assert(!GROUPED || (!FUSED && !ACC32 && !BATCHED), "grouped wgrad: plain bf16 mode");
   constexpr int BN = tile_n<FUSED>();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = aligned_smem(smem_raw);
@@ -367,6 +437,10 @@ wgrad_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
 
   const int n_tiles = g.N / BM;  // tiles along the rows of G
   const int k_tiles = (g.K + BN - 1) / BN;  // tiles along the columns of G (K % 128 == 0: a last tile may be half)
+  if constexpr (GROUPED) {
+    grouped_wgrad_roles<BN>(smem, pipe, &tmap_a, &tmap_b, g, n_tiles, k_tiles);
+    return;
+  }
   const int num_tiles = n_tiles * k_tiles * (BATCHED ? g.experts : 1);
   const UnitSched sched = make_sched(num_tiles, gridDim.x, g.ksplit);
   const int num_units = sched.num_units;
@@ -521,6 +595,25 @@ void launch_wgrad_bf16_batched(const void* dy, const void* x, void* gout, int64_
       persistent_grid(E * (N / BM) * ((K + BN - 1) / BN), sm_count), kGemmThreads, Tile<BN>::kSmemBytes, stream,
       "wgrad_bf16_batched", make_tmap_mn(dy, E * Mb, N, N), make_tmap_mn(x, E * Mb, K, K),
       wgrad_args(gout, Mb, N, K, K, 1, gscale, 0.0f, E), WgradComm{});
+}
+
+bool wgrad_bf16_grouped_supported(int64_t E, int64_t R, int64_t N, int64_t K, const void* dy, const void* x,
+                                  const void* g, const void* counts) {
+  return E > 0 && E <= kMaxGroups && R % BM == 0 && wgrad_bf16_supported(R, N, K, dy, x, g, N, K, K) &&
+         (reinterpret_cast<uintptr_t>(counts) & 3u) == 0 &&
+         E * N / BM * ((K + tile_n<false>() - 1) / tile_n<false>()) < (1ll << 31) && E * N < (1ll << 31);
+}
+
+void launch_wgrad_bf16_grouped(const void* dy, const void* x, void* gout, const int* counts, int64_t E, int64_t R,
+                               int64_t N, int64_t K, int sm_count, cudaStream_t stream, const float* gscale) {
+  M4T_CHECK(wgrad_bf16_grouped_supported(E, R, N, K, dy, x, gout, counts),
+            "unsupported shape/alignment for the grouped wgrad (N % 128, K % 128, rows % 128, 16-byte-aligned operands)");
+  constexpr int BN = tile_n<false>();
+  WgradArgs g = wgrad_args(gout, R, N, K, K, 1, gscale, 0.0f, E);
+  g.group_counts = counts;
+  launch_kernel<wgrad_bf16_wgmma_kernel<false, false, false, true>>(
+      persistent_grid(E * (N / BM) * ((K + BN - 1) / BN), sm_count), kGemmThreads, Tile<BN>::kSmemBytes + kGroupTableBytes,
+      stream, "wgrad_bf16_grouped", make_tmap_mn(dy, R, N, N), make_tmap_mn(x, R, K, K), g, WgradComm{});
 }
 
 int64_t fused_wgrad_tiles(int64_t N, int64_t K) { return (N / BM) * (K / tile_n<true>()); }

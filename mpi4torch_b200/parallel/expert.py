@@ -12,7 +12,8 @@ produced by autograd.
 ``dispatch_to_experts`` / ``combine_from_experts`` do the same per expert: ``experts_per_rank`` experts live on
 every rank and each has ``capacity`` slots per source rank, so the exchange is ONE ``Alltoall`` of an
 ``[E, P, capacity, d]`` tensor.  :class:`ExpertParallelMLP` is the mixture-of-experts feed-forward layer built on
-them and on :func:`mpi4torch_b200.ops.expert_mlp`.
+them and on :func:`mpi4torch_b200.ops.expert_mlp`, or, dropless (``capacity=None``), on
+:func:`mpi4torch_b200.ops.grouped_expert_mlp`.
 """
 from __future__ import annotations
 
@@ -23,7 +24,7 @@ import torch
 import torch.nn.functional as F
 
 import mpi4torch_b200 as m4t
-from mpi4torch_b200.ops.expert_mlp import expert_mlp
+from mpi4torch_b200.ops.expert_mlp import expert_group_starts, expert_mlp, grouped_expert_mlp, grouped_rows
 
 from .tensor_parallel import replicated_input
 
@@ -182,9 +183,17 @@ class ExpertParallelMLP(torch.nn.Module):
     slots being zero rows.  The experts run on the batched kernels (:func:`mpi4torch_b200.ops.expert_mlp`) when
     ``expert_mlp_supported`` holds: bf16 CUDA tensors, ``d_model`` and ``hidden`` multiples of 128, and
     ``P * C % 128 == 0``, i.e. ``C % 128 == 0`` at one rank and ``C % 16 == 0`` at eight.  Otherwise the same math
-    runs as the torch composition."""
+    runs as the torch composition.
 
-    def __init__(self, d_model: int, hidden: int, experts_per_rank: int, capacity: int, comm=None, top_k: int = 1,
+    ``capacity=None``: dropless routing.  No pair is dropped and each expert computes exactly the rows routed to it,
+    on the grouped kernels (:func:`mpi4torch_b200.ops.grouped_expert_mlp`, when ``grouped_expert_mlp_supported``
+    holds: bf16 CUDA tensors, ``d_model`` and ``hidden`` multiples of 128).  At one rank the pairs go straight into
+    the grouped layout with no host synchronisation.  At several ranks one ``Alltoall`` exchanges the per-expert
+    pair counts and one ``Allreduce(MAX)``, read on the host, sets the exchange's capacity to the largest count; the
+    exchange then moves the padded ``[E, P, C, d_model]`` buffer and the received rows are packed into the grouped
+    layout."""
+
+    def __init__(self, d_model: int, hidden: int, experts_per_rank: int, capacity, comm=None, top_k: int = 1,
                  dtype=torch.bfloat16, device="cpu", seed: int = 0):
         super().__init__()
         self.comm = m4t.COMM_WORLD if comm is None else comm
@@ -215,8 +224,47 @@ class ExpertParallelMLP(torch.nn.Module):
         router = replicated_input(self.router, c)
         probs = torch.softmax(F.linear(x.to(router.dtype), router), dim=-1)  # [T, P * E]
         gate, choice = probs.topk(self.top_k, dim=-1)                          # [T, k]
-        received, routing = dispatch_to_experts(x, choice, self.experts_per_rank, self.capacity, c)
-        y = expert_mlp(received, self.w1, self.b1, self.w2, self.b2)          # [E, P * C, d_model]
-        back = combine_from_experts(y, routing, c)                             # [T, k, d_model]
+        if self.capacity is None:
+            back = self._dropless(x, choice)
+            dropped = torch.zeros(choice.shape, dtype=torch.bool, device=choice.device)
+        else:
+            received, routing = dispatch_to_experts(x, choice, self.experts_per_rank, self.capacity, c)
+            y = expert_mlp(received, self.w1, self.b1, self.w2, self.b2)          # [E, P * C, d_model]
+            back = combine_from_experts(y, routing, c)                             # [T, k, d_model]
+            dropped = routing.slot < 0
         out = (gate.unsqueeze(-1) * back.to(gate.dtype)).sum(1).to(x.dtype)
-        return out, MoERouting(probs=probs, expert=choice, dropped=routing.slot < 0)
+        return out, MoERouting(probs=probs, expert=choice, dropped=dropped)
+
+    def _experts(self, xg, counts):
+        return grouped_expert_mlp(xg, counts.to(torch.int32), self.w1, self.b1, self.w2, self.b2)
+
+    def _dropless(self, x: torch.Tensor, choice: torch.Tensor) -> torch.Tensor:
+        """[T, k, d_model]: every (token, choice) pair's expert output, no pair dropped."""
+        c = self.comm
+        P, E = c.size, self.experts_per_rank
+        T, k = choice.shape
+        d = x.shape[1]
+        if P == 1:
+            # pair i = j * T + t (choice-major, as the slots of dispatch_to_experts) goes to row
+            # start[expert] + (pairs before it with the same expert)
+            flat = choice.t().reshape(-1)
+            onehot = F.one_hot(flat, E)
+            rows = expert_group_starts(onehot.sum(0))[flat] + (onehot.cumsum(0) - onehot).gather(1, flat[:, None])[:, 0]
+            R = grouped_rows(T * k, E)
+            xg = x.new_zeros((R, d)).index_add(0, rows, x.repeat(k, 1))
+            y = self._experts(xg, onehot.sum(0))
+            return y[rows].reshape(k, T, d).transpose(0, 1)
+        send = F.one_hot(choice.reshape(-1), P * E).sum(0).to(torch.int32)     # [P * E] pairs for each global expert
+        recv = _exchange(send.reshape(P, 1, E), c).reshape(P, E)               # [P(source), E] pairs received
+        C = max(int(c.Allreduce(send.max().reshape(1), m4t.MPI_MAX).item()), 1)  # the one host read
+        received, routing = dispatch_to_experts(x, choice, E, C, c)            # [E, P * C, d], nothing dropped
+        counts = recv.sum(0)                                                   # [E] rows of each local expert
+        before = (torch.cumsum(recv, 0) - recv).t()                            # [E, P] rows from earlier sources
+        s = torch.arange(C, device=x.device)
+        dst = expert_group_starts(counts)[:, None, None] + before[:, :, None] + s  # [E, P, C] row in the grouped layout
+        R = grouped_rows(E * P * C, E)
+        dst = torch.where(s < recv.t()[:, :, None], dst, R).reshape(-1)       # empty slots -> a scratch row R
+        xg = received.new_zeros((R + 1, d)).index_add(0, dst, received.reshape(-1, d))[:R]
+        y = self._experts(xg, counts)
+        processed = torch.cat([y, y.new_zeros((1, d))])[dst].reshape(E, P * C, d)
+        return combine_from_experts(processed, routing, c)
