@@ -563,9 +563,10 @@ bool bf16_2d(const Tensor& t) {
   return t.is_cuda() && t.dim() == 2 && t.scalar_type() == at::kBFloat16 && t.is_contiguous();
 }
 
+// The kernels read the counts as int32 words: a 4-byte-aligned base.
 bool counts_ok(const Tensor& counts, const Tensor& like) {
   return counts.is_cuda() && counts.device() == like.device() && counts.dim() == 1 && counts.scalar_type() == at::kInt &&
-         counts.is_contiguous() && counts.numel() > 0;
+         counts.is_contiguous() && counts.numel() > 0 && (reinterpret_cast<uintptr_t>(counts.data_ptr()) & 3u) == 0;
 }
 
 // x [R, K] @ w [E, N, K]^T by groups, and the bias [E, N] (contiguous fp32, 8-byte aligned) when given.

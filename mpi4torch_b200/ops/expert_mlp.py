@@ -58,6 +58,14 @@ def expert_mlp_supported(x: torch.Tensor, w1: torch.Tensor, b1: torch.Tensor, w2
                 and ops.batched_gemm_tn_supported(x.new_empty((E, M, w1.shape[1])), w2, b2))
 
 
+def _kernel_grad(dy: torch.Tensor) -> torch.Tensor:
+    """The upstream gradient as the backward kernels read it: contiguous, with a 16-byte-aligned base.  The forward
+    never sees it, so it may be e.g. the expanded gradient of a sum, or a slice of a larger buffer at an odd offset,
+    which ``.contiguous()`` returns unchanged."""
+    dy = dy.contiguous()
+    return dy if dy.data_ptr() % 16 == 0 else dy.clone()
+
+
 class _ExpertMLP(torch.autograd.Function):
     """Kernel path of :func:`expert_mlp`.  Backward takes the bf16 upstream gradient dy and fills plain gradients;
     an input that needs no gradient gets none, and no launch is spent on it."""
@@ -75,7 +83,7 @@ class _ExpertMLP(torch.autograd.Function):
         x, w1, w2, h, z = ctx.saved_tensors
         ops = _ops()
         need = ctx.needs_input_grad
-        dy = dy.contiguous()  # e.g. the expanded gradient of a sum
+        dy = _kernel_grad(dy)
         gx = gw1 = gb1 = gw2 = gb2 = None
         if need[0] or need[1] or need[2]:
             dz, dz_part = ops.batched_gemm_nn_gelu_backward(dy, w2, z)
@@ -184,7 +192,7 @@ class _GroupedExpertMLP(torch.autograd.Function):
         x, counts, w1, w2, h, z = ctx.saved_tensors
         ops = _ops()
         need = ctx.needs_input_grad
-        dy = dy.contiguous()
+        dy = _kernel_grad(dy)
         gx = gw1 = gb1 = gw2 = gb2 = None
         if need[0] or need[2] or need[3]:
             dz, dz_part = ops.grouped_gemm_nn_gelu_backward(dy, w2, z, counts)

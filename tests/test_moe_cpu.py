@@ -43,6 +43,31 @@ def test_composition_matches_float64(dtype, tol):
         assert err <= tol * max(1.0, float(ref.abs().max())), f"{dtype} {name}: {err}"
 
 
+@pytest.mark.parametrize("grouped", [False, True])
+def test_composition_takes_a_misaligned_upstream_gradient(grouped):
+    """An upstream gradient that is contiguous but sits one element into its buffer (a base the kernels could not
+    read) gives the gradients of an aligned copy of it."""
+    from mpi4torch_b200.ops import grouped_expert_mlp
+
+    E, M, D, H, O = 3, 10, 6, 12, 5
+    x, w1, b1, w2, b2 = _inputs(E, M, D, H, O, torch.float64)
+    args = (x.reshape(E * M, D), torch.tensor([4, 0, 9], dtype=torch.int32)) if grouped else (x,)
+    node = grouped_expert_mlp if grouped else expert_mlp
+    grads = []
+    for offset in (0, 1):
+        ins = [t.clone().requires_grad_() for t in (args[0], w1, b1, w2, b2)]
+        y = node(ins[0], *args[1:], *ins[1:])
+        dy = torch.randn(y.shape, generator=torch.Generator().manual_seed(2), dtype=torch.float64)
+        buf = torch.full((y.numel() + 1,), float("nan"), dtype=torch.float64)
+        view = buf[offset:offset + y.numel()].view(y.shape)
+        view.copy_(dy)
+        assert view.is_contiguous() and view.storage_offset() == offset
+        y.backward(view)
+        grads.append([t.grad for t in ins])
+    for name, got, ref in zip(("x", "w1", "b1", "w2", "b2"), grads[1], grads[0]):
+        torch.testing.assert_close(got, ref, rtol=1e-12, atol=1e-12, msg=name)
+
+
 def test_expert_mlp_rejects_mismatched_shapes():
     x, w1, b1, w2, b2 = _inputs(2, 4, 6, 8, 5, torch.float64)
     with pytest.raises(ValueError):
