@@ -24,6 +24,20 @@ Uniform routing gives every expert M pairs.  Skewed routing is seeded: expert 0 
 mean load and the others share the rest at random.  FLOP/s count the routed rows only.
 
     python benchmarks/moe_step.py --routing skewed [--shapes small,large]
+
+With ``--update`` naming more than ``grad`` it compares how the expert parameters are trained, one training step of
+the experts each (x requires a gradient too, as in a layer):
+
+* ``grad``: the plain node, bf16 ``.grad`` of the weights, then the torch SGD pass ``p -= lr * p.grad`` it implies;
+* ``sgd``: ``optimizer=InBackwardSGD(lr)``, the SGD step in the wgrad kernels' epilogue, no ``.grad``;
+* ``accumulate``: ``accumulator=AccumulatedSGD(lr)``, one micro-batch added into the fp32 buffers (its ``step()``,
+  once per K micro-batches, is not in the timed window).
+
+It runs the large batched shape and the skewed grouped case (expert 0 at ``--skew`` times the mean load) and reports
+the step medians (arms alternated), the per-kernel device times of a separate profiler run and the peak device memory
+of one step of each arm.
+
+    python benchmarks/moe_step.py --update grad,sgd,accumulate
 """
 import argparse
 import json
@@ -39,8 +53,8 @@ sys.path.insert(0, ROOT)
 import mpi4torch_b200 as m4t  # noqa: E402
 from benchmarks.fp8_linear_step import kernel_times  # noqa: E402
 from benchmarks.mlp_step import card, time_ms  # noqa: E402
-from mpi4torch_b200.ops import (expert_group_starts, expert_mlp, expert_mlp_supported, grouped_expert_mlp,  # noqa: E402
-                                 grouped_expert_mlp_supported)
+from mpi4torch_b200.ops import (AccumulatedSGD, InBackwardSGD, expert_group_starts, expert_mlp,  # noqa: E402
+                                 expert_mlp_supported, grouped_expert_mlp, grouped_expert_mlp_supported)
 from mpi4torch_b200.ops.expert_mlp import grouped_rows  # noqa: E402
 
 SHAPES = {"small": (8, 256, 1024, 4096), "large": (8, 1024, 4096, 16384)}  # E, M, D, H (O = D)
@@ -189,6 +203,87 @@ def routing_main(a):
         print(json.dumps(res), flush=True)
 
 
+UPDATE_LR = 1e-6  # small enough that thousands of timed steps leave the weights' magnitudes unchanged
+
+
+def make_update_arms(kind, E, M, D, H, counts, modes):
+    """One training step of the experts per call, in each update mode of `modes`."""
+    g = torch.Generator(device="cuda").manual_seed(0)
+    r = lambda *s, scale=1.0: (torch.randn(*s, generator=g, device="cuda") * scale)  # noqa: E731
+    init = [r(E, H, D, scale=D ** -0.5).to(torch.bfloat16), r(E, H, scale=0.1),
+            r(E, D, H, scale=H ** -0.5).to(torch.bfloat16), r(E, D, scale=0.1)]
+    if kind == "batched":
+        x, dy = r(E, M, D).to(torch.bfloat16), r(E, M, D).to(torch.bfloat16)
+        node = lambda xx, ps, **u: expert_mlp(xx, *ps, **u)  # noqa: E731
+        assert expert_mlp_supported(x, *init)
+    else:
+        cnt = torch.tensor(counts, dtype=torch.int32, device="cuda")
+        R = grouped_rows(sum(counts), E)
+        x, dy = torch.zeros(R, D, device="cuda", dtype=torch.bfloat16), torch.zeros(R, D, device="cuda", dtype=torch.bfloat16)
+        for s, c in zip(expert_group_starts(cnt).tolist(), counts):
+            x[s:s + c], dy[s:s + c] = r(c, D).to(torch.bfloat16), r(c, D).to(torch.bfloat16)
+        node = lambda xx, ps, **u: grouped_expert_mlp(xx, cnt, *ps, **u)  # noqa: E731
+        assert grouped_expert_mlp_supported(x, cnt, *init)
+    arms = {}
+    for mode in modes:
+        ps = [t.clone().requires_grad_() for t in init]
+        xm = x.clone().requires_grad_()
+        update = {"sgd": {"optimizer": InBackwardSGD(UPDATE_LR)},
+                  "accumulate": {"accumulator": AccumulatedSGD(UPDATE_LR)}}.get(mode, {})
+
+        def step(ps=ps, xm=xm, update=update, mode=mode):
+            node(xm, ps, **update).backward(dy)
+            xm.grad = None
+            if mode == "grad":
+                with torch.no_grad():
+                    for p in ps:
+                        p.add_(p.grad, alpha=-UPDATE_LR)
+                        p.grad = None
+
+        arms[mode] = step
+    return arms
+
+
+def update_main(a, modes):
+    skewed = route_counts(*SHAPES["large"][:2], "skewed", a.skew)
+    for kind, counts in (("batched", None), ("grouped", skewed)):
+        E, M, D, H = SHAPES["large"]
+        res = {"card": card(), "update": kind, "shape": {"E": E, "M": M, "D": D, "H": H, "O": D}, "lr": UPDATE_LR}
+        if counts:
+            res["counts"] = counts
+        arms = make_update_arms(kind, E, M, D, H, counts, modes)
+        peak = {}
+        for k, fn in arms.items():  # one step each, measured alone, after the first (the buffers are allocated)
+            fn()
+            torch.cuda.synchronize()
+            torch.cuda.reset_peak_memory_stats()
+            base = torch.cuda.memory_allocated()
+            fn()
+            torch.cuda.synchronize()
+            peak[k] = {"peak_mib": round(torch.cuda.max_memory_allocated() / 2 ** 20, 1),
+                       "peak_above_resident_mib": round((torch.cuda.max_memory_allocated() - base) / 2 ** 20, 1)}
+        for fn in arms.values():
+            for _ in range(a.warmup):
+                fn()
+        torch.cuda.synchronize()
+        times = {k: [] for k in arms}
+        names = list(arms)
+        for rep in range(a.reps):
+            for k in (names if rep % 2 == 0 else names[::-1]):
+                times[k].append(time_ms(arms[k], a.steps))
+        res["step_ms"] = {k: {"min": round(min(v), 4), "median": round(statistics.median(v), 4), "max": round(max(v), 4)}
+                          for k, v in times.items()}
+        res["memory"] = peak
+        for k in arms:
+            kt = kernel_times(arms[k], 10, None, k)
+            merged = {}
+            for name, ms in kt.items():
+                merged[short(name)] = merged.get(short(name), 0.0) + ms
+            res[f"kernels_ms_{k}"] = {n: round(v, 4) for n, v in sorted(merged.items(), key=lambda kv: -kv[1])}
+            res[f"device_ms_{k}"] = round(sum(merged.values()), 4)
+        print(json.dumps(res), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--shapes", default="small,large")
@@ -199,10 +294,18 @@ def main():
     ap.add_argument("--routing", choices=("uniform", "skewed"), default=None,
                     help="compare the grouped (dropless) node with the batched one under this routing")
     ap.add_argument("--skew", type=float, default=4.0, help="skewed routing: max / mean load")
+    ap.add_argument("--update", default="grad",
+                    help="comma-separated update modes from grad, sgd, accumulate; grad alone: the comparison above")
     a = ap.parse_args()
+    modes = a.update.split(",")
+    if not set(modes) <= {"grad", "sgd", "accumulate"}:
+        raise SystemExit("--update takes grad, sgd and accumulate")
     if not torch.cuda.is_available():
         raise SystemExit("moe_step.py measures on the GPU; none is visible")
     assert m4t.COMM_WORLD.size == 1 and m4t.cuda_backend_ready()
+    if modes != ["grad"]:
+        update_main(a, modes)
+        return
     if a.routing:
         routing_main(a)
         return

@@ -689,6 +689,100 @@ Tensor grouped_column_sum(const Tensor& in, const Tensor& counts) {
   return out;
 }
 
+// ---- expert weight updates inside the expert wgrads (in-backward SGD, fp32 micro-batch accumulation) --------------
+// The weight or buffer is written in place, tile by tile, by the one CTA that computes the tile, and the wgrad never
+// reads it: the update is safe unless it shares memory with dy or x, which the predicates reject.
+bool disjoint(const Tensor& a, const Tensor& b) {
+  const auto* pa = static_cast<const char*>(a.data_ptr());
+  const auto* pb = static_cast<const char*>(b.data_ptr());
+  return pa + a.nbytes() <= pb || pb + b.nbytes() <= pa;
+}
+
+// `out` [E, N, K] contiguous, of dtype `dt`, on the operands' device, 16-byte aligned, disjoint from dy and x.
+bool expert_out_ok(const Tensor& out, at::ScalarType dt, int64_t E, const Tensor& dy, const Tensor& x, int64_t N,
+                   int64_t K) {
+  return out.is_cuda() && out.device() == x.device() && out.dim() == 3 && out.scalar_type() == dt &&
+         out.is_contiguous() && out.size(0) == E && out.size(1) == N && out.size(2) == K && (reinterpret_cast<uintptr_t>(out.data_ptr()) & 15u) == 0 &&
+         disjoint(out, dy) && disjoint(out, x);
+}
+
+// w [E, N, K] bf16 (or buf fp32) updated from dy [E, M, N] and x [E, M, K].
+bool batched_wgrad_update_ok(const Tensor& out, at::ScalarType dt, const Tensor& dy, const Tensor& x) {
+  return batched_wgrad_bf16_ok(dy, x) && expert_out_ok(out, dt, dy.size(0), dy, x, dy.size(2), x.size(2));
+}
+
+bool batched_wgrad_sgd_ok(const Tensor& w, const Tensor& dy, const Tensor& x) {
+  return batched_wgrad_update_ok(w, at::kBFloat16, dy, x);
+}
+
+bool batched_wgrad_accumulate_ok(const Tensor& buf, const Tensor& dy, const Tensor& x) {
+  return batched_wgrad_update_ok(buf, at::kFloat, dy, x);
+}
+
+// w [E, N, K] bf16 (or buf fp32) updated from dy [R, N] and x [R, K] by groups of counts [E].
+bool grouped_wgrad_update_ok(const Tensor& out, at::ScalarType dt, const Tensor& dy, const Tensor& x,
+                             const Tensor& counts) {
+  return grouped_wgrad_bf16_ok(dy, x, counts) && expert_out_ok(out, dt, counts.size(0), dy, x, dy.size(1), x.size(1)) &&
+         disjoint(out, counts);
+}
+
+bool grouped_wgrad_sgd_ok(const Tensor& w, const Tensor& dy, const Tensor& x, const Tensor& counts) {
+  return grouped_wgrad_update_ok(w, at::kBFloat16, dy, x, counts);
+}
+
+bool grouped_wgrad_accumulate_ok(const Tensor& buf, const Tensor& dy, const Tensor& x, const Tensor& counts) {
+  return grouped_wgrad_update_ok(buf, at::kFloat, dy, x, counts);
+}
+
+const char* kUpdateRules = ", the batched_wgrad_bf16 (or grouped_wgrad_bf16) operand rules, and the updated tensor "
+                           "contiguous and 16-byte aligned on the same device, sharing no memory with dy, x or counts";
+
+// w_e <- bf16(w_e + scale * grad_scale * dy_e^T @ x_e): the SGD step of every expert as the batched wgrad's epilogue.
+void batched_wgrad_sgd_(Tensor w, const Tensor& dy, const Tensor& x, double scale, const c10::optional<Tensor>& grad_scale) {
+  TORCH_CHECK(batched_wgrad_sgd_ok(w, dy, x), "mpi4torch_b200: batched_wgrad_sgd_ needs bf16 w [E, N, K], dy [E, M, N] "
+              "and x [E, M, K]", kUpdateRules);
+  TORCH_CHECK(scale != 0.0, "mpi4torch_b200: batched_wgrad_sgd_ needs a non-zero scale");
+  c10::cuda::CUDAGuard guard(x.device());
+  std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
+  launch_wgrad_bf16_batched(dy.data_ptr(), x.data_ptr(), w.data_ptr(), dy.size(0), dy.size(1), dy.size(2), x.size(2),
+                            sm_count(), stream_of(x), grad_scale_ptr(grad_scale, x), static_cast<float>(scale));
+}
+
+// buf_e <- fmaf(grad_scale, dy_e^T @ x_e, buf_e) in fp32, every expert in one launch.
+void batched_wgrad_accumulate_(Tensor buf, const Tensor& dy, const Tensor& x, const c10::optional<Tensor>& grad_scale) {
+  TORCH_CHECK(batched_wgrad_accumulate_ok(buf, dy, x), "mpi4torch_b200: batched_wgrad_accumulate_ needs fp32 buf "
+              "[E, N, K], bf16 dy [E, M, N] and x [E, M, K]", kUpdateRules);
+  c10::cuda::CUDAGuard guard(x.device());
+  std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
+  launch_wgrad_accumulate_batched(dy.data_ptr(), x.data_ptr(), buf.data_ptr<float>(), dy.size(0), dy.size(1), dy.size(2),
+                                  x.size(2), sm_count(), stream_of(x), grad_scale_ptr(grad_scale, x));
+}
+
+// w_e <- bf16(w_e + scale * grad_scale * G_e) over group e's rows; an empty group's w_e is not written.
+void grouped_wgrad_sgd_(Tensor w, const Tensor& dy, const Tensor& x, const Tensor& counts, double scale,
+                        const c10::optional<Tensor>& grad_scale) {
+  TORCH_CHECK(grouped_wgrad_sgd_ok(w, dy, x, counts), "mpi4torch_b200: grouped_wgrad_sgd_ needs bf16 w [E, N, K], "
+              "dy [R, N] and x [R, K], int32 counts [E]", kUpdateRules);
+  TORCH_CHECK(scale != 0.0, "mpi4torch_b200: grouped_wgrad_sgd_ needs a non-zero scale");
+  c10::cuda::CUDAGuard guard(x.device());
+  std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
+  launch_wgrad_bf16_grouped(dy.data_ptr(), x.data_ptr(), w.data_ptr(), counts.data_ptr<int>(), counts.size(0), dy.size(0),
+                            dy.size(1), x.size(1), sm_count(), stream_of(x), grad_scale_ptr(grad_scale, x),
+                            static_cast<float>(scale));
+}
+
+// buf_e <- fmaf(grad_scale, G_e, buf_e) in fp32 over group e's rows; an empty group's buf_e is not written.
+void grouped_wgrad_accumulate_(Tensor buf, const Tensor& dy, const Tensor& x, const Tensor& counts,
+                               const c10::optional<Tensor>& grad_scale) {
+  TORCH_CHECK(grouped_wgrad_accumulate_ok(buf, dy, x, counts), "mpi4torch_b200: grouped_wgrad_accumulate_ needs fp32 "
+              "buf [E, N, K], bf16 dy [R, N] and x [R, K], int32 counts [E]", kUpdateRules);
+  c10::cuda::CUDAGuard guard(x.device());
+  std::lock_guard<std::recursive_mutex> g(World::instance().mutex());
+  launch_wgrad_accumulate_grouped(dy.data_ptr(), x.data_ptr(), buf.data_ptr<float>(), counts.data_ptr<int>(),
+                                  counts.size(0), dy.size(0), dy.size(1), x.size(1), sm_count(), stream_of(x),
+                                  grad_scale_ptr(grad_scale, x));
+}
+
 // ---- FP8 linear layer (gemm_fp8.cu) ------------------------------------------------------------------------------
 bool fp8_e5m2(c10::string_view fmt) {
   TORCH_CHECK(fmt == "e4m3" || fmt == "e5m2", "mpi4torch_b200: the fp8 format must be 'e4m3' or 'e5m2'");
@@ -845,6 +939,19 @@ TORCH_LIBRARY_FRAGMENT(mpi4torch_b200, m) {
   m.def("grouped_gemm_nn(Tensor a, Tensor b, Tensor counts) -> Tensor", &grouped_gemm_nn);
   m.def("grouped_wgrad_bf16(Tensor dy, Tensor x, Tensor counts, Tensor? grad_scale=None) -> Tensor", &grouped_wgrad_bf16);
   m.def("grouped_column_sum(Tensor partials, Tensor counts) -> Tensor", &grouped_column_sum);
+  m.def("batched_wgrad_sgd_supported(Tensor w, Tensor dy, Tensor x) -> bool", &batched_wgrad_sgd_ok);
+  m.def("batched_wgrad_accumulate_supported(Tensor buf, Tensor dy, Tensor x) -> bool", &batched_wgrad_accumulate_ok);
+  m.def("grouped_wgrad_sgd_supported(Tensor w, Tensor dy, Tensor x, Tensor counts) -> bool", &grouped_wgrad_sgd_ok);
+  m.def("grouped_wgrad_accumulate_supported(Tensor buf, Tensor dy, Tensor x, Tensor counts) -> bool",
+        &grouped_wgrad_accumulate_ok);
+  m.def("batched_wgrad_sgd_(Tensor(a!) w, Tensor dy, Tensor x, float scale, Tensor? grad_scale=None) -> ()",
+        &batched_wgrad_sgd_);
+  m.def("batched_wgrad_accumulate_(Tensor(a!) buf, Tensor dy, Tensor x, Tensor? grad_scale=None) -> ()",
+        &batched_wgrad_accumulate_);
+  m.def("grouped_wgrad_sgd_(Tensor(a!) w, Tensor dy, Tensor x, Tensor counts, float scale, Tensor? grad_scale=None) -> ()",
+        &grouped_wgrad_sgd_);
+  m.def("grouped_wgrad_accumulate_(Tensor(a!) buf, Tensor dy, Tensor x, Tensor counts, Tensor? grad_scale=None) -> ()",
+        &grouped_wgrad_accumulate_);
   m.def("linear_bias_gelu_forward(Tensor x, Tensor w, Tensor b) -> (Tensor, Tensor)", &linear_bias_gelu_forward);
   m.def("linear_bias_mse_forward_local(Tensor x, Tensor w, Tensor b, Tensor target, float loss_scale, float grad_scale) "
         "-> (Tensor, Tensor, Tensor)",

@@ -223,8 +223,12 @@ void launch_column_sum_batched(const float* partial, int64_t E, int64_t rows, in
 // G_e [N, K] = gscale * dY_e^T X_e with dY [E, Mb, N], X [E, Mb, K], G [E, N, K]; the rules of wgrad_bf16_supported.
 bool wgrad_bf16_batched_supported(int64_t E, int64_t Mb, int64_t N, int64_t K, const void* dy, const void* x,
                                   const void* g);
+// axpy != 0: the SGD step g_e <- bf16(g_e + axpy * gscale * dY_e^T X_e) in place of G (as launch_wgrad_bf16).
 void launch_wgrad_bf16_batched(const void* dy, const void* x, void* g, int64_t E, int64_t Mb, int64_t N, int64_t K,
-                               int sm_count, cudaStream_t stream, const float* gscale = nullptr);
+                               int sm_count, cudaStream_t stream, const float* gscale = nullptr, float axpy = 0.0f);
+// acc [E, N, K] (fp32) <- fmaf(gscale, dY_e^T X_e, acc_e), as launch_wgrad_accumulate per expert.
+void launch_wgrad_accumulate_batched(const void* dy, const void* x, float* acc, int64_t E, int64_t Mb, int64_t N,
+                                     int64_t K, int sm_count, cudaStream_t stream, const float* gscale = nullptr);
 
 // ---- grouped experts (gemm_wgmma.cu, wgrad_wgmma.cu; DESIGN §4.4) -------------------------------------------------
 // E experts with row counts `counts` [E] (int32, read on the device only) share one [R, .] operand in the grouped
@@ -251,8 +255,14 @@ void launch_column_sum_grouped(const void* in, bool bf16_rows, const int* counts
 // G_e [N, K] = gscale * dY_e^T X_e over group e's rows of dY [R, N] and X [R, K]; G [E, N, K], zero for an empty group.
 bool wgrad_bf16_grouped_supported(int64_t E, int64_t R, int64_t N, int64_t K, const void* dy, const void* x,
                                   const void* g, const void* counts);
+// axpy != 0: the SGD step g_e <- bf16(g_e + axpy * gscale * G_e); an empty group's g_e is not written.
 void launch_wgrad_bf16_grouped(const void* dy, const void* x, void* g, const int* counts, int64_t E, int64_t R,
-                               int64_t N, int64_t K, int sm_count, cudaStream_t stream, const float* gscale = nullptr);
+                               int64_t N, int64_t K, int sm_count, cudaStream_t stream, const float* gscale = nullptr,
+                               float axpy = 0.0f);
+// acc [E, N, K] (fp32) <- fmaf(gscale, G_e, acc_e); an empty group's acc_e is not written.
+void launch_wgrad_accumulate_grouped(const void* dy, const void* x, float* acc, const int* counts, int64_t E, int64_t R,
+                                     int64_t N, int64_t K, int sm_count, cudaStream_t stream,
+                                     const float* gscale = nullptr);
 
 // ---- FP8 training of the linear layer (gemm_fp8.cu, DESIGN §4.4) ---------------------------------------------
 // Per-tensor power-of-two scaling: amax of a bf16 [rows, cols] matrix (leading dimension ld) -> *amax_bits (the bit

@@ -354,8 +354,10 @@ __device__ __forceinline__ void acc32_epilogue(const float (&acc)[BN / 2], char*
 }
 
 // The grouped wgrad (wgrad_bf16_wgmma_kernel with GROUPED): tile t of E * n_tiles * k_tiles is (expert, n, k) as in the
-// batched kernel, contracted over the expert's rows [128 pfx[e], end[e]) of the grouped layout.
-template <int BN>
+// batched kernel, contracted over the expert's rows [128 pfx[e], end[e]) of the grouped layout.  The epilogue is chosen
+// at compile time: G (bf16), the SGD step W <- bf16(W + g.axpy * gscale * G) (SGD), or the fp32 accumulation (ACC32).
+// In the two updating modes an expert without rows stores nothing, so its weight or buffer keeps its exact bits.
+template <int BN, bool ACC32, bool SGD>
 __device__ __forceinline__ void grouped_wgrad_roles(uint8_t* smem, Pipe* pipe, const CUtensorMap* tmap_a,
                                                     const CUtensorMap* tmap_b, const WgradArgs& g, int n_tiles,
                                                     int k_tiles) {
@@ -389,7 +391,8 @@ __device__ __forceinline__ void grouped_wgrad_roles(uint8_t* smem, Pipe* pipe, c
     int stage = 0;
     uint32_t phase = 0;
     float acc[BN / 2];
-    const float gs = g.gscale ? __ldg(g.gscale) : 1.0f;
+    // SGD: the plain kernel's axpy scale, (gscale * axpy), so both round the same products
+    const float gs = SGD ? (g.gscale ? __ldg(g.gscale) : 1.0f) * g.axpy : (g.gscale ? __ldg(g.gscale) : 1.0f);
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
       const int n_blk = t / k_tiles;
       const int k_blk = t - n_blk * k_tiles;
@@ -398,9 +401,11 @@ __device__ __forceinline__ void grouped_wgrad_roles(uint8_t* smem, Pipe* pipe, c
       const int kbs = (rows + BK - 1) / BK;
       if (kbs > 0) {
         mma_tile<true, true, BN, true>(acc, smem, pipe, stage, phase, kbs, wgi, rows - (kbs - 1) * BK);
-        bf16_epilogue<BN>(acc, static_cast<char*>(g.out), g.ldo, g.K, gs, false, n_blk, k_blk, wgi);
+        if constexpr (ACC32) acc32_epilogue<BN>(acc, static_cast<char*>(g.out), g.ldo, g.K, gs, n_blk, k_blk, wgi);
+        else bf16_epilogue<BN>(acc, static_cast<char*>(g.out), g.ldo, g.K, gs, SGD, n_blk, k_blk, wgi);
         continue;
       }
+      if constexpr (ACC32 || SGD) continue;  // updating modes: an expert without rows leaves its tile untouched
       // an expert without rows: a zero gradient (zeroing acc instead makes ptxas spill it)
       const int cols = min(BN, g.K - k_blk * BN);
 #pragma unroll 1
@@ -415,19 +420,23 @@ __device__ __forceinline__ void grouped_wgrad_roles(uint8_t* smem, Pipe* pipe, c
   __syncthreads();
 }
 
-// ACC32 (plain mode only): out is an fp32 [N, K] buffer and the epilogue is out <- fmaf(gscale, G, out), the
+// ACC32 (not FUSED): out is an fp32 [N, K] buffer and the epilogue is out <- fmaf(gscale, G, out), the
 // gradient accumulation of micro-batches.  A compile-time mode, so the other instantiations are unchanged.
-// BATCHED (plain mode only): E = g.experts problems G_e = dY_e^T X_e of the same shape, with dY [E Mb, N], X [E Mb, K]
+// BATCHED (not FUSED): E = g.experts problems G_e = dY_e^T X_e of the same shape, with dY [E Mb, N], X [E Mb, K]
 // and out [E N, K] stacked.  Tile rows of the stacked output run over E * N / 128 blocks: block n_blk belongs to
 // expert n_blk / (N / 128), whose contraction rows start at row expert * Mb of both operands.
-// GROUPED (plain mode only): the same tiles and output, with dY [Mb, N] and X [Mb, K] in the grouped layout of
+// GROUPED (not FUSED, not BATCHED): the same tiles and output, with dY [Mb, N] and X [Mb, K] in the grouped layout of
 // g.group_counts over Mb rows (GroupTable).  Expert e contracts over the ceil(rows_e / 64) k-blocks from its first
-// row; the last one's rows past the group are zeroed in both operands, and an expert without rows stores zeros.
-template <bool FUSED, bool ACC32 = false, bool BATCHED = false, bool GROUPED = false>
+// row; the last one's rows past the group are zeroed in both operands, and an expert without rows stores zeros (G) or
+// nothing (ACC32, SGD).
+// SGD (GROUPED only): the SGD epilogue out <- bf16(out + axpy * gscale * G) as a compile-time mode; the other kernels
+// select it at run time through g.axpy.
+template <bool FUSED, bool ACC32 = false, bool BATCHED = false, bool GROUPED = false, bool SGD = false>
 __global__ void __launch_bounds__(kGemmThreads + (FUSED ? kCommWarps * 32 : 0), 1)
 wgrad_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                         const WgradArgs g, const WgradComm wc) {
-  static_assert(!GROUPED || (!FUSED && !ACC32 && !BATCHED), "grouped wgrad: plain bf16 mode");
+  static_assert(!GROUPED || (!FUSED && !BATCHED && !(ACC32 && SGD)), "grouped wgrad: one epilogue, not fused");
+  static_assert(!SGD || GROUPED, "the compile-time SGD epilogue is the grouped kernel's");
   constexpr int BN = tile_n<FUSED>();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = aligned_smem(smem_raw);
@@ -438,7 +447,7 @@ wgrad_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid
   const int n_tiles = g.N / BM;  // tiles along the rows of G
   const int k_tiles = (g.K + BN - 1) / BN;  // tiles along the columns of G (K % 128 == 0: a last tile may be half)
   if constexpr (GROUPED) {
-    grouped_wgrad_roles<BN>(smem, pipe, &tmap_a, &tmap_b, g, n_tiles, k_tiles);
+    grouped_wgrad_roles<BN, ACC32, SGD>(smem, pipe, &tmap_a, &tmap_b, g, n_tiles, k_tiles);
     return;
   }
   const int num_tiles = n_tiles * k_tiles * (BATCHED ? g.experts : 1);
@@ -587,14 +596,25 @@ bool wgrad_bf16_batched_supported(int64_t E, int64_t Mb, int64_t N, int64_t K, c
 }
 
 void launch_wgrad_bf16_batched(const void* dy, const void* x, void* gout, int64_t E, int64_t Mb, int64_t N, int64_t K,
-                               int sm_count, cudaStream_t stream, const float* gscale) {
+                               int sm_count, cudaStream_t stream, const float* gscale, float axpy) {
   M4T_CHECK(wgrad_bf16_batched_supported(E, Mb, N, K, dy, x, gout),
             "unsupported shape/alignment for the batched wgrad (N % 128, K % 128, batch % 64, 16-byte-aligned operands)");
   constexpr int BN = tile_n<false>();
   launch_kernel<wgrad_bf16_wgmma_kernel<false, false, true>>(
       persistent_grid(E * (N / BM) * ((K + BN - 1) / BN), sm_count), kGemmThreads, Tile<BN>::kSmemBytes, stream,
-      "wgrad_bf16_batched", make_tmap_mn(dy, E * Mb, N, N), make_tmap_mn(x, E * Mb, K, K),
-      wgrad_args(gout, Mb, N, K, K, 1, gscale, 0.0f, E), WgradComm{});
+      axpy != 0.0f ? "wgrad_sgd_batched" : "wgrad_bf16_batched", make_tmap_mn(dy, E * Mb, N, N),
+      make_tmap_mn(x, E * Mb, K, K), wgrad_args(gout, Mb, N, K, K, 1, gscale, axpy, E), WgradComm{});
+}
+
+void launch_wgrad_accumulate_batched(const void* dy, const void* x, float* acc, int64_t E, int64_t Mb, int64_t N,
+                                     int64_t K, int sm_count, cudaStream_t stream, const float* gscale) {
+  M4T_CHECK(wgrad_bf16_batched_supported(E, Mb, N, K, dy, x, acc),
+            "unsupported shape/alignment for the batched wgrad (N % 128, K % 128, batch % 64, 16-byte-aligned operands)");
+  constexpr int BN = tile_n<false>();
+  launch_kernel<wgrad_bf16_wgmma_kernel<false, true, true>>(
+      persistent_grid(E * (N / BM) * ((K + BN - 1) / BN), sm_count), kGemmThreads, Tile<BN>::kSmemBytes, stream,
+      "wgrad_accumulate_batched", make_tmap_mn(dy, E * Mb, N, N), make_tmap_mn(x, E * Mb, K, K),
+      wgrad_args(acc, Mb, N, K, K, 1, gscale, 0.0f, E), WgradComm{});
 }
 
 bool wgrad_bf16_grouped_supported(int64_t E, int64_t R, int64_t N, int64_t K, const void* dy, const void* x,
@@ -604,16 +624,33 @@ bool wgrad_bf16_grouped_supported(int64_t E, int64_t R, int64_t N, int64_t K, co
          E * N / BM * ((K + tile_n<false>() - 1) / tile_n<false>()) < (1ll << 31) && E * N < (1ll << 31);
 }
 
-void launch_wgrad_bf16_grouped(const void* dy, const void* x, void* gout, const int* counts, int64_t E, int64_t R,
-                               int64_t N, int64_t K, int sm_count, cudaStream_t stream, const float* gscale) {
-  M4T_CHECK(wgrad_bf16_grouped_supported(E, R, N, K, dy, x, gout, counts),
+namespace {
+// Mode of the grouped wgrad: G, the SGD step (axpy != 0) or the fp32 accumulation.
+template <bool ACC32, bool SGD>
+void launch_grouped(const char* what, const void* dy, const void* x, void* out, const int* counts, int64_t E, int64_t R,
+                    int64_t N, int64_t K, int sm_count, cudaStream_t stream, const float* gscale, float axpy) {
+  M4T_CHECK(wgrad_bf16_grouped_supported(E, R, N, K, dy, x, out, counts),
             "unsupported shape/alignment for the grouped wgrad (N % 128, K % 128, rows % 128, 16-byte-aligned operands)");
   constexpr int BN = tile_n<false>();
-  WgradArgs g = wgrad_args(gout, R, N, K, K, 1, gscale, 0.0f, E);
+  WgradArgs g = wgrad_args(out, R, N, K, K, 1, gscale, axpy, E);
   g.group_counts = counts;
-  launch_kernel<wgrad_bf16_wgmma_kernel<false, false, false, true>>(
+  launch_kernel<wgrad_bf16_wgmma_kernel<false, ACC32, false, true, SGD>>(
       persistent_grid(E * (N / BM) * ((K + BN - 1) / BN), sm_count), kGemmThreads, Tile<BN>::kSmemBytes + kGroupTableBytes,
-      stream, "wgrad_bf16_grouped", make_tmap_mn(dy, R, N, N), make_tmap_mn(x, R, K, K), g, WgradComm{});
+      stream, what, make_tmap_mn(dy, R, N, N), make_tmap_mn(x, R, K, K), g, WgradComm{});
+}
+}  // namespace
+
+void launch_wgrad_bf16_grouped(const void* dy, const void* x, void* gout, const int* counts, int64_t E, int64_t R,
+                               int64_t N, int64_t K, int sm_count, cudaStream_t stream, const float* gscale, float axpy) {
+  if (axpy != 0.0f)
+    launch_grouped<false, true>("wgrad_sgd_grouped", dy, x, gout, counts, E, R, N, K, sm_count, stream, gscale, axpy);
+  else
+    launch_grouped<false, false>("wgrad_bf16_grouped", dy, x, gout, counts, E, R, N, K, sm_count, stream, gscale, 0.0f);
+}
+
+void launch_wgrad_accumulate_grouped(const void* dy, const void* x, float* acc, const int* counts, int64_t E, int64_t R,
+                                     int64_t N, int64_t K, int sm_count, cudaStream_t stream, const float* gscale) {
+  launch_grouped<true, false>("wgrad_accumulate_grouped", dy, x, acc, counts, E, R, N, K, sm_count, stream, gscale, 0.0f);
 }
 
 int64_t fused_wgrad_tiles(int64_t N, int64_t K) { return (N / BM) * (K / tile_n<true>()); }

@@ -94,6 +94,10 @@ class AccumulatedSGD:
     ``p += AllreduceFused(buf, SUM, -lr / P)``: one parameter-sized collective per parameter and step, summed in a
     fixed order, so every rank ends with the same bits.
 
+    Owned parameters (the experts of ``expert_mlp`` / ``grouped_expert_mlp``, which live on one rank only) register
+    with ``buffer(param, None)``: :meth:`step` applies ``p -= lr * buf`` to them locally, with no collective.  One
+    accumulator can hold replicated and owned parameters together.
+
     The parameter averages ``mean_ranks(p)`` that the forwards read are computed once per step (by the first
     forward) and reused by the later forwards of the same step.  ``updates`` counts the calls of :meth:`step`; a
     backward whose forward came before the last :meth:`step` raises ``RuntimeError``.  Several forwards before one
@@ -107,7 +111,8 @@ class AccumulatedSGD:
         self._avgs = {}  # id(param) -> (param, version, average)
 
     def buffer(self, param: torch.Tensor, comm) -> torch.Tensor:
-        """The gradient buffer of ``param`` (allocated zeroed at the first call)."""
+        """The gradient buffer of ``param`` (allocated zeroed at the first call).  ``comm`` is the communicator over
+        which ``param`` is replicated, or ``None`` for a parameter this rank owns alone."""
         entry = self._bufs.get(id(param))
         if entry is None or entry[0] is not param:
             dtype = torch.float32 if param.dtype in (torch.bfloat16, torch.float16) else param.dtype
@@ -153,10 +158,13 @@ class AccumulatedSGD:
 
     @torch.no_grad()
     def step(self) -> None:
-        """One SGD update per buffered parameter from the sum of every rank's buffer; zeroes the buffers."""
+        """One SGD update per buffered parameter from the sum of every rank's buffer (an owned parameter: from its
+        own buffer); zeroes the buffers."""
         for p, buf, comm in self._bufs.values():
-            upd = comm.AllreduceFused(buf, m4t.MPI_SUM, -self.lr / comm.size, None)
-            p.add_(upd)
+            if comm is None:
+                p.add_(buf, alpha=-self.lr)
+            else:
+                p.add_(comm.AllreduceFused(buf, m4t.MPI_SUM, -self.lr / comm.size, None))
             buf.zero_()
         self.updates += 1
         self._avgs.clear()
@@ -184,6 +192,13 @@ def accumulated_average(acc: AccumulatedSGD, comm, param: torch.Tensor) -> torch
     copy: ``step()`` updates the parameter in place while a stale node may still hold the average."""
     avg = acc.average(comm, param, (lambda: param.detach().clone()) if comm.size == 1 else None)
     return _AccumulateGrad.apply(param, avg, acc, comm) if param.requires_grad else avg
+
+
+def owned_accumulated(acc: AccumulatedSGD, param: torch.Tensor) -> torch.Tensor:
+    """``param`` as a composition path reads it when ``acc`` accumulates the gradient of a parameter this rank owns
+    (no collective, ``step()`` updates it locally): a copy, since ``step()`` updates the parameter in place while a
+    stale node may still hold it."""
+    return _AccumulateGrad.apply(param, param.detach().clone(), acc, None) if param.requires_grad else param
 
 
 def _wgrad_accumulate(buf: torch.Tensor, gy: torch.Tensor, x: torch.Tensor, gscale: Optional[torch.Tensor]) -> None:

@@ -191,7 +191,13 @@ class ExpertParallelMLP(torch.nn.Module):
     the grouped layout with no host synchronisation.  At several ranks one ``Alltoall`` exchanges the per-expert
     pair counts and one ``Allreduce(MAX)``, read on the host, sets the exchange's capacity to the largest count; the
     exchange then moves the padded ``[E, P, C, d_model]`` buffer and the received rows are packed into the grouped
-    layout."""
+    layout.
+
+    ``forward(x, optimizer=None, accumulator=None)`` trains the experts inside backward, in both routing modes and at
+    any P (see :func:`mpi4torch_b200.ops.expert_mlp`): with an ``InBackwardSGD`` the expert weights and biases are
+    updated by the backward itself (kernel path only), with an ``AccumulatedSGD`` their gradients go into its fp32
+    buffers and ``step()`` applies them, with no collective either way.  The experts then get no ``.grad``.  The
+    router is tiny, replicated and fp32: it keeps its ``.grad`` in both modes, for the caller's own update."""
 
     def __init__(self, d_model: int, hidden: int, experts_per_rank: int, capacity, comm=None, top_k: int = 1,
                  dtype=torch.bfloat16, device="cpu", seed: int = 0):
@@ -219,26 +225,27 @@ class ExpertParallelMLP(torch.nn.Module):
         self.w2 = torch.nn.Parameter(w2[mine].to(dtype).to(device).contiguous())
         self.b2 = torch.nn.Parameter(b2[mine].to(fdt).to(device).contiguous())
 
-    def forward(self, x: torch.Tensor):
+    def forward(self, x: torch.Tensor, optimizer=None, accumulator=None):
         c = self.comm
+        update = {"optimizer": optimizer, "accumulator": accumulator}
         router = replicated_input(self.router, c)
         probs = torch.softmax(F.linear(x.to(router.dtype), router), dim=-1)  # [T, P * E]
         gate, choice = probs.topk(self.top_k, dim=-1)                          # [T, k]
         if self.capacity is None:
-            back = self._dropless(x, choice)
+            back = self._dropless(x, choice, update)
             dropped = torch.zeros(choice.shape, dtype=torch.bool, device=choice.device)
         else:
             received, routing = dispatch_to_experts(x, choice, self.experts_per_rank, self.capacity, c)
-            y = expert_mlp(received, self.w1, self.b1, self.w2, self.b2)          # [E, P * C, d_model]
+            y = expert_mlp(received, self.w1, self.b1, self.w2, self.b2, **update)  # [E, P * C, d_model]
             back = combine_from_experts(y, routing, c)                             # [T, k, d_model]
             dropped = routing.slot < 0
         out = (gate.unsqueeze(-1) * back.to(gate.dtype)).sum(1).to(x.dtype)
         return out, MoERouting(probs=probs, expert=choice, dropped=dropped)
 
-    def _experts(self, xg, counts):
-        return grouped_expert_mlp(xg, counts.to(torch.int32), self.w1, self.b1, self.w2, self.b2)
+    def _experts(self, xg, counts, update):
+        return grouped_expert_mlp(xg, counts.to(torch.int32), self.w1, self.b1, self.w2, self.b2, **update)
 
-    def _dropless(self, x: torch.Tensor, choice: torch.Tensor) -> torch.Tensor:
+    def _dropless(self, x: torch.Tensor, choice: torch.Tensor, update) -> torch.Tensor:
         """[T, k, d_model]: every (token, choice) pair's expert output, no pair dropped."""
         c = self.comm
         P, E = c.size, self.experts_per_rank
@@ -252,7 +259,7 @@ class ExpertParallelMLP(torch.nn.Module):
             rows = expert_group_starts(onehot.sum(0))[flat] + (onehot.cumsum(0) - onehot).gather(1, flat[:, None])[:, 0]
             R = grouped_rows(T * k, E)
             xg = x.new_zeros((R, d)).index_add(0, rows, x.repeat(k, 1))
-            y = self._experts(xg, onehot.sum(0))
+            y = self._experts(xg, onehot.sum(0), update)
             return y[rows].reshape(k, T, d).transpose(0, 1)
         send = F.one_hot(choice.reshape(-1), P * E).sum(0).to(torch.int32)     # [P * E] pairs for each global expert
         recv = _exchange(send.reshape(P, 1, E), c).reshape(P, E)               # [P(source), E] pairs received
@@ -265,6 +272,6 @@ class ExpertParallelMLP(torch.nn.Module):
         R = grouped_rows(E * P * C, E)
         dst = torch.where(s < recv.t()[:, :, None], dst, R).reshape(-1)       # empty slots -> a scratch row R
         xg = received.new_zeros((R + 1, d)).index_add(0, dst, received.reshape(-1, d))[:R]
-        y = self._experts(xg, counts)
+        y = self._experts(xg, counts, update)
         processed = torch.cat([y, y.new_zeros((1, d))])[dst].reshape(E, P * C, d)
         return combine_from_experts(processed, routing, c)
