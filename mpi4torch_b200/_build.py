@@ -42,6 +42,7 @@ _SOURCES = [
     "api/comm_raw.cpp",
     "api/autograd_ops.cpp",
     "api/fused_ops.cpp",
+    "api/virtual_ranks.cpp",
     "api/bindings.cpp",
 ]
 

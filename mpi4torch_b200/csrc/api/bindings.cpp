@@ -68,6 +68,8 @@ void activate_nvlink_transport() { World::instance().set_host_staging(false); }
 
 }  // namespace
 
+void register_virtual_ranks(py::module& m);  // virtual_ranks.cpp
+
 TORCH_LIBRARY(mpi4torch_b200, m) {
   m.class_<Communicator>("Communicator")
       .def("GetRank", &Communicator::GetRank)
@@ -199,6 +201,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     PullPlan p = plan_repartition(rank, size, before, after, cur, nw);
     return py::make_tuple(jobs_to_py(p.jobs), p.stage_elems, p.out_elems);
   });
+  register_virtual_ranks(m);
   m.def("check_device_error", [] {
     World& w = World::instance();
     if (w.cuda_ready()) w.cuda()->check_device_error();
